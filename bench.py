@@ -21,12 +21,11 @@ e2e   : same call with PINNED HOST tensors -- H2D copy of the batch and D2H read
         semantics; reported beside it as `sync_loss`).
 roofline : the fused rollout kernel alone, timed with CUDA events on its launch stream inside the library
         (gops_b200_plan_enable_timing).  Compute bound by design (SURVEY.md 8(d)): `achieved` = algorithmic TFLOP/s,
-        `peak` = tensor roof for FP32-accurate (BF16x3) GEMMs = measured BURST bf16 peak / 6 (the kernel is timed alone);
-        FP32-FFMA, HBM, raw-bf16 and sustained-peak fractions beside it.
+        `peak` = tensor roof for FP32-accurate (BF16x3) GEMMs = bf16 peak / 6 (MEASURED_PEAKS.json when present, else the
+        H100 SXM data sheet); FP32-FFMA, HBM, raw-bf16 and sustained-peak fractions beside it.
 cpu_baseline : the UNMODIFIED reference's `alg.local_update` (oracle/_ref, kind "reference") on the host cores, on a
         bounded sample of the same workload -- or the oracle port (kind "port") if the reference tree is absent.
-gpu_eager_baseline : the unmodified reference with use_gpu=True on the same B200 (PyTorch eager; SURVEY 8(d)'s
-        "existing Blackwell path").
+gpu_eager_baseline : the unmodified reference with use_gpu=True on the same GPU (PyTorch eager).
 configs : the other BASELINE.json configurations, each one timed update (device-resident inputs, L2 flushed between
         iterations) with its own kernel path and roofline line.
 """
@@ -48,8 +47,10 @@ OBS_DIM, ACT_DIM, HID = 6, 1, 64
 MAC = (OBS_DIM + 1) * HID + HID * HID + HID * ACT_DIM          # 4608
 FLOP_PER_ENV_STEP = 6 * MAC + 1500                             # SURVEY.md 8(d): MLP fwd+bwd + dynamics
 BYTES_PER_ENV_STEP = (OBS_DIM * 4 + 4) / H                     # obs + done read once per sample
-L2_BYTES = 126 * 1024 * 1024
+L2_BYTES = 50 * 1024 * 1024                                     # H100 SXM L2
 GLOBAL_BATCH = 1 << 18
+# roofline fallbacks when MEASURED_PEAKS.json is absent: NVIDIA's H100 SXM data sheet (700 W card), dense rates
+H100_HBM_GBS, H100_BF16_TFLOPS, H100_SM_MAX_MHZ = 3350.0, 989.0, 1980.0
 
 
 def alg_kwargs(env_id="pyth_idpendulum", algorithm="FHADP", hid=HID, act="gelu", obs_dim=OBS_DIM, act_dim=ACT_DIM, **kw):
@@ -67,7 +68,7 @@ def alg_kwargs(env_id="pyth_idpendulum", algorithm="FHADP", hid=HID, act="gelu",
 
 
 class ClockSampler:
-    """nvidia-smi sampling DURING the timed region (B200_PROFILING.md clocks line): one `nvidia-smi -lms 100`
+    """nvidia-smi sampling DURING the timed region (SM clock, power, throttle reasons): one `nvidia-smi -lms 100`
     child process started before and killed after the region."""
 
     QUERY = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
@@ -238,7 +239,20 @@ class Harness:
         return float(ms.item()), kms, launches
 
 
-def measure_c1(hx, batch_per_gpu, K, W, want_kernel=True, want_e2e=True, want_sync=True):
+def dump_outputs(alg, dump_dir):
+    """What the last timed update handed its caller: the updated policy parameters, the gradient it applied and the
+    result tail [loss | v-mean | #done | pad], as float32 .npy files."""
+    import numpy as np
+    os.makedirs(dump_dir, exist_ok=True)
+    fp = alg.networks.policy.flat_params
+    gbuf = fp.gbuf.detach().float().cpu().numpy()
+    params = np.concatenate([p.detach().float().cpu().numpy().ravel() for p in alg.networks.policy.parameters()])
+    np.save(os.path.join(dump_dir, "policy_params.npy"), params.astype(np.float32))
+    np.save(os.path.join(dump_dir, "policy_grad.npy"), gbuf[:params.size].astype(np.float32))
+    np.save(os.path.join(dump_dir, "result_tail.npy"), gbuf[params.size:].astype(np.float32))
+
+
+def measure_c1(hx, batch_per_gpu, K, W, want_kernel=True, want_e2e=True, want_sync=True, dump_dir=None):
     """The C1 update on this rank's shard: returns dict(value-side timings, kernel ms, e2e timings, launches)."""
     import torch
     from gops_b200.create_pkg.create_alg import create_alg
@@ -264,6 +278,8 @@ def measure_c1(hx, batch_per_gpu, K, W, want_kernel=True, want_e2e=True, want_sy
     sampler.start()
     out["ms_total"], _, out["launches"] = hx.timed(alg, dev_sets, K)
     out["clocks"] = sampler.stop()
+    if dump_dir is not None and hx.rank == 0:
+        dump_outputs(alg, dump_dir)
     if want_sync:
         alg.loss_lag = 0
         hx.timed(alg, dev_sets, 2)
@@ -279,7 +295,7 @@ def measure_c1(hx, batch_per_gpu, K, W, want_kernel=True, want_e2e=True, want_sy
     return out
 
 
-PATH_TEXT = {"tc": "tcgen05: BF16x3 UMMA for every dense product, weight gradients accumulate in TMEM",
+PATH_TEXT = {"tc": "wgmma: BF16x3 warpgroup MMAs for every dense product, FP32 weight-gradient accumulation",
              "mma": "mma.sync 3xTF32 (64-wide nets) / FP32 FFMA (256-wide nets)"}
 
 
@@ -293,9 +309,9 @@ def secondary_configs(hx, peaks, K=10, W=3):
     from gops_b200.trainer import device_sampler as ds
     dev = hx.dev
     flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-    burst = peaks.get("bf16_tflops", 1700.0)
+    burst = peaks.get("bf16_tflops", H100_BF16_TFLOPS)
     n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
-    ffma_peak = n_sm * 128 * 2 * peaks.get("sm_max_mhz", 1965.0) * 1e6 / 1e12
+    ffma_peak = n_sm * 128 * 2 * peaks.get("sm_max_mhz", H100_SM_MAX_MHZ) * 1e6 / 1e12
     rows = []
 
     def run(name, kw, data, horizon, flop_pev, flop_pim, set_params=None):
@@ -352,7 +368,7 @@ def secondary_configs(hx, peaks, K=10, W=3):
         alg_kwargs("veh3dof_tracking", "FHADP", 256, "elu", 6 + 4 * 60, 2, pre_horizon=60, policy_learning_rate=1e-3),
         d, 60, None, 7.8e5)
     # C4 DSAC idpendulum, [256,256,256] gelu, minibatch 8192 from the on-device replay buffer: one update = 5 network
-    # evaluations + 3 back-propagations on the layer-wise tcgen05 MLP (2.7 MFLOP algorithmic per sample, SURVEY 8(f) N1)
+    # evaluations + 3 back-propagations on the layer-wise wgmma MLP (2.7 MFLOP algorithmic per sample, SURVEY 8(f) N1)
     try:
         from gops_b200.trainer.device_buffer import DeviceReplayBuffer
         torch.manual_seed(0)
@@ -411,6 +427,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-configs", action="store_true")
     ap.add_argument("--no-eager", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed update of the main measurement as DIR/<name>.npy")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -435,7 +453,7 @@ def main():
     Bglobal = args.global_batch
     per_gpu_strong = Bglobal // world
     main_b = per_gpu_strong if args.scaling == "strong" else Bglobal
-    m = measure_c1(hx, main_b, K, W)
+    m = measure_c1(hx, main_b, K, W, dump_dir=args.dump_outputs)
     other = None
     if world > 1:      # the other scaling mode, same run (value side only)
         other_b = Bglobal if args.scaling == "strong" else per_gpu_strong
@@ -449,34 +467,27 @@ def main():
                 peaks = json.load(f)
         except Exception:
             pass
-        peak_src = "MEASURED_PEAKS.json" if peaks else "fallback (B200_PROFILING.md)"
-        hbm_peak = peaks.get("hbm_gbs", 6650.0)
-        burst = peaks.get("bf16_tflops", 1700.0)
-        sustained = peaks.get("bf16_tflops_sustained", 1400.0)
+        peak_src = "MEASURED_PEAKS.json" if peaks else "H100 SXM data sheet (not measured)"
+        hbm_peak = peaks.get("hbm_gbs", H100_HBM_GBS)
+        burst = peaks.get("bf16_tflops", H100_BF16_TFLOPS)
+        sustained = peaks.get("bf16_tflops_sustained", burst)
         env_steps = main_b * world * H
         value = env_steps * K / (m["ms_total"] * 1e-3)
         e2e = env_steps * K / (m["ms_e2e"] * 1e-3)
         k_ms = statistics.mean(m["kernel_ms"])
         clocks = m["clocks"]
-        sm_mhz = clocks["sm_mhz"] or peaks.get("sm_max_mhz", 1965.0)
+        sm_mhz = clocks["sm_mhz"] or peaks.get("sm_max_mhz", H100_SM_MAX_MHZ)
         n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
         fp32_peak = n_sm * 128 * 2 * sm_mhz * 1e6 / 1e12
         ach_tflops = main_b * H * FLOP_PER_ENV_STEP / (k_ms * 1e-3) / 1e12
         ach_gbs = main_b * H * BYTES_PER_ENV_STEP / (k_ms * 1e-3) / 1e9
-        traffic = None
-        tfile = os.path.join(ROOT, "profiles", "traffic.json")
-        if os.path.exists(tfile):
-            try:
-                traffic = json.load(open(tfile)).get("rollout_kernel_dram_bytes_per_launch")
-            except Exception:
-                pass
         path = m["launch"]["kernel_path"]
         # FP32-accurate tensor roof: BF16x3 = six bf16 MMAs per product (tc path), 3xTF32 = three TF32 MMAs at half the
         # bf16 rate (mma path): both = bf16 peak / 6.  The kernel is event-timed alone -> burst peak.
         tens_roof = burst / 6.0
         m["launch"]["kernel_path_text"] = PATH_TEXT.get(path, path)
         roof = {"bound": "tensor", "achieved": ach_tflops, "peak": tens_roof, "unit": "TFLOP/s",
-                "frac": ach_tflops / tens_roof, "traffic": traffic,
+                "frac": ach_tflops / tens_roof,
                 "peak_source": f"{peak_src} bf16_tflops (burst: kernel timed alone) / 6 (six bf16 MMAs per FP32-accurate product)",
                 "frac_of_sustained_peak": ach_tflops / (sustained / 6.0),
                 "kernel_ms": k_ms, "kernel_share_of_step": k_ms * K / m["ms_total"],

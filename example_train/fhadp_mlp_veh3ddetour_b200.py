@@ -2,7 +2,7 @@
 """Interior-point FHADP on the vehicle detour task, trained entirely on the GPU (counterpart of the reference's
 example_train/fhadp/fhadp_mlp_veh3ddetour_serial.py: FHADPInterior, veh3dof_tracking_detour, pre_horizon 30,
 [256, 256] elu policy, lr 1e-3).  States, references and the surrounding vehicle's predictions are drawn on the device
-(gops_b200/trainer/device_sampler.py); the update runs on the layer-wise tcgen05 path (csrc/lw_detour.cuh)."""
+(gops_b200/trainer/device_sampler.py); the update runs on the layer-wise wgmma path (csrc/lw_detour.cuh)."""
 import argparse
 import os
 import sys

@@ -1,4 +1,4 @@
-"""gops_b200: B200-native (sm_100a CUDA) implementation of GOPS's batched model-rollout +
+"""gops_b200: H100-native (sm_90a CUDA) implementation of GOPS's batched model-rollout +
 ADP-update hot path behind GOPS's own plugin API.
 
 Layout mirrors the reference package for the modules on the path:

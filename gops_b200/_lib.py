@@ -1,7 +1,7 @@
 """ctypes binding of libgops_b200.so (C ABI in include/gops_b200.h).
 
 There is no CPU fallback: if the shared library is missing or a call fails, a RuntimeError is
-raised.  Build it with `python -c "import __graft_entry__ as g; g.build()"` (nvcc, sm_100a).
+raised.  Build it with `python -c "import __graft_entry__ as g; g.build()"` (nvcc, sm_90a).
 """
 import ctypes as C
 import os

@@ -1,7 +1,7 @@
-"""Distributional Soft Actor-Critic (DSAC), B200 edition.
+"""Distributional Soft Actor-Critic (DSAC), H100 edition.
 
 Same plugin surface as the reference (gops/algorithm/dsac.py: ApproxContainer :34-65, DSAC :68-290).  One update =
-five network evaluations and three back-propagations, all on the layer-wise tcgen05 MLP (csrc/dense_tc.cu, BF16x3),
+five network evaluations and three back-propagations, all on the layer-wise wgmma MLP (csrc/dense_tc.cu, BF16x3),
 joined by the library's fused elementwise kernels (csrc/dsac.cu: reparameterised tanh-Gaussian sampling and its
 log-density, clipped-TD distributional critic loss, actor loss -- each with its hand-derived gradient), the fused Adam
 and Polyak kernels.  No autograd graph, no host round trip until the scalars of the update are read back.

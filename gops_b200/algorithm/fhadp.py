@@ -1,4 +1,4 @@
-"""Finite-horizon approximate dynamic programming (FHADP), B200 edition.
+"""Finite-horizon approximate dynamic programming (FHADP), H100 edition.
 
 Same plugin surface as the reference (gops/algorithm/fhadp.py: ApproxContainer :32-55, FHADP
 :58-125).  `_compute_gradient` replaces the python horizon loop + autograd of

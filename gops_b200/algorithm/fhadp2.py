@@ -1,8 +1,8 @@
 """FHADP2: finite-horizon ADP with an OPEN-LOOP policy (reference gops/algorithm/fhadp2.py:20-121).
 
 `FiniteHorizonFullPolicy` maps obs_0 to the whole action sequence; the loss is the negative discounted return of the
-model rollout under that sequence (fhadp2.py:98-121).  Here: one tcgen05 policy evaluation (all H actions), the fused
-per-step rollout kernels (forward and hand-derived adjoint, csrc/lw_rollout.cuh), one tcgen05 policy backward -- the
+model rollout under that sequence (fhadp2.py:98-121).  Here: one wgmma policy evaluation (all H actions), the fused
+per-step rollout kernels (forward and hand-derived adjoint, csrc/lw_rollout.cuh), one wgmma policy backward -- the
 gradient lands in the policy's flat `.grad`, followed by the NCCL all-reduce (torchrun) and the fused Adam step."""
 __all__ = ["FHADP2"]
 

@@ -1,4 +1,4 @@
-"""Infinite-horizon approximate dynamic programming (INFADP), B200 edition.
+"""Infinite-horizon approximate dynamic programming (INFADP), H100 edition.
 
 Same plugin surface as the reference (gops/algorithm/infadp.py: ApproxContainer :31-64, INFADP
 :67-213).  The value branch (`__compute_loss_v` :159-186) and the policy branch

@@ -1,8 +1,8 @@
-"""MLP approximate functions of the ADP hot path, B200 edition.
+"""MLP approximate functions of the ADP hot path, H100 edition.
 
 Same constructor kwargs, class names, `state_dict` keys and init as the reference
 (gops/apprfunc/mlp.py: mlp() :36-41, DetermPolicy :50-77, FiniteHorizonPolicy :80-111,
-StateValue :309-329); `forward` runs the fused sm_100a inference kernel
+StateValue :309-329); `forward` runs the fused sm_90a inference kernels
 (`gops_b200_mlp_forward`) instead of nn.Sequential.  Training never calls `forward`: the
 algorithms hand the flat parameter vector to the fused rollout kernel.
 """
@@ -118,7 +118,7 @@ class FiniteHorizonPolicy(_FusedMlp):
 
 class FiniteHorizonFullPolicy(nn.Module, Action_Distribution):
     """Open-loop finite-horizon policy (reference mlp.py:114-145): ONE evaluation on obs emits the actions of all
-    `pre_horizon` steps; `forward` returns the first one.  Evaluated by the layer-wise tcgen05 MLP
+    `pre_horizon` steps; `forward` returns the first one.  Evaluated by the layer-wise wgmma MLP
     (gops_b200_mlpnet_*); trained by FHADP2 through the fused open-loop rollout."""
 
     def __init__(self, **kwargs):
@@ -171,7 +171,7 @@ class FiniteHorizonFullPolicy(nn.Module, Action_Distribution):
 
 
 class _LayerwiseNet(nn.Module):
-    """A general `mlp()` network (any depth, widths <= 256) evaluated by the layer-wise tcgen05 MLP."""
+    """A general `mlp()` network (any depth, widths <= 256) evaluated by the layer-wise wgmma MLP."""
 
     _attr = "net"
 

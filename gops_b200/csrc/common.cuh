@@ -1,4 +1,4 @@
-// Device-side helpers shared by the gops_b200 kernels (sm_100a).
+// Device-side helpers shared by the gops_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -73,17 +73,29 @@ __device__ __forceinline__ void gelu_parts(float x, float& cdf, float& pdf) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// Packed FP32 pairs (sm_100: FFMA2 / FMUL2 / FADD2 do two IEEE-rn operations per issue slot).  The epilogues are
-// issue-bound element-wise code over 16 independent columns per thread, so adjacent columns are processed as pairs:
-// same operations, same rounding, same order as the scalar forms above -- results are bit-identical.
+// FP32 pairs: the epilogues process adjacent columns as (lo, hi) pairs held in one 64-bit register pair.  sm_90 has no
+// packed FP32 arithmetic, so each pair operation is two scalar IEEE-rn operations in the same order (the pair form keeps
+// the epilogue code shared and lets the compiler interleave the two independent chains).
 // ---------------------------------------------------------------------------------------------
 namespace f32x2 {
 typedef unsigned long long u64;
 __device__ __forceinline__ u64 pk(float lo, float hi) { u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
 __device__ __forceinline__ void upk(u64 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ u64 fma(u64 a, u64 b, u64 c) { u64 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
-__device__ __forceinline__ u64 mul(u64 a, u64 b) { u64 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ u64 add(u64 a, u64 b) { u64 r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
+__device__ __forceinline__ u64 fma(u64 a, u64 b, u64 c) {
+  float a0, a1, b0, b1, c0, c1;
+  upk(a, a0, a1); upk(b, b0, b1); upk(c, c0, c1);
+  return pk(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
+}
+__device__ __forceinline__ u64 mul(u64 a, u64 b) {
+  float a0, a1, b0, b1;
+  upk(a, a0, a1); upk(b, b0, b1);
+  return pk(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
+}
+__device__ __forceinline__ u64 add(u64 a, u64 b) {
+  float a0, a1, b0, b1;
+  upk(a, a0, a1); upk(b, b0, b1);
+  return pk(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
+}
 __device__ __forceinline__ u64 rep(float c) { return pk(c, c); }
 __device__ __forceinline__ u64 ld(const float* p) { return *reinterpret_cast<const u64*>(p); }      // 8-byte aligned pair
 }  // namespace f32x2

@@ -1,4 +1,4 @@
-// C ABI of the generic tcgen05 dense-layer path (include/gops_b200.h, section "layer-wise MLP"): a trainable MLP of
+// C ABI of the generic wgmma dense-layer path (include/gops_b200.h, section "layer-wise MLP"): a trainable MLP of
 // any depth (widths <= 256 per layer) evaluated layer by layer with the kernels of dense_tc.cuh.  Used by the wide-net
 // FHADP path, DSAC and FHADP2; the fused rollout kernels remain the path for 64-wide nets with small inputs.
 #include "gops_b200.h"
@@ -105,7 +105,7 @@ int gops_b200_mlpnet_create(const int32_t* sizes, int32_t n_sizes, int32_t hidde
     delete net;
     return dense_fail("no CUDA device");
   }
-  if (prop.major < 10) { delete net; return dense_fail("gops_b200 requires an sm_100a (B200) device"); }
+  if (prop.major != 9 || prop.minor != 0) { delete net; return dense_fail("gops_b200 is built for sm_90a and needs an H100-class (sm_90) device"); }
   net->sm_count = prop.multiProcessorCount;
   net->max_smem = (int)prop.sharedMemPerBlockOptin;
   net->nl = n_sizes - 1;

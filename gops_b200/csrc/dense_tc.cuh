@@ -1,4 +1,4 @@
-// Generic dense layers on tcgen05 / TMEM in FP32-accurate BF16x3 arithmetic: the building block of the layer-wise paths
+// Generic dense layers on the Hopper warpgroup tensor cores (wgmma) in FP32-accurate BF16x3 arithmetic: the building block of the layer-wise paths
 // (wide nets: FHADP veh3dof_tracking [256,256]; DSAC [256,256,256]; FHADP2's open-loop policy) where a whole-horizon
 // fusion does not fit one SM's shared memory.
 //
@@ -6,14 +6,14 @@
 //   dgrad     dX[r][k] = (sum_n dY[r][n] W[n][k]) * M[r][k]          (M: saved act' of the layer below, optional)
 //   wgrad     dW[n][k] = sum_r dY[r][n] X[r][k]                       (row-split partials, fixed-order reduction)
 //
-// All three are C = A . B^T GEMMs with M = 128 rows per CTA on the tensor core, operands as bf16 planes in the
-// no-swizzle canonical layout plane[chunk = col/8][row][8] (the layout of the fused rollout kernels, umma.cuh):
+// All three are C = A . B^T GEMMs with M = 128 rows per CTA (two warpgroups of 64 rows), operands as bf16 planes in the
+// no-swizzle canonical layout plane[chunk = col/8][row][8] (wgmma.cuh):
 //   * activations (fp32, row-major in HBM) are converted by the CTA while it stages them: thread = (8-column chunk, row),
 //     one 32-byte global read, one 16-byte shared store per plane (conflict-free: consecutive lanes = consecutive rows);
 //   * weights are pre-split once per update by pack_dense_kernel into exactly the shared-memory image of each
 //     (column split, K slice) and fetched with one TMA bulk copy per slice;
-//   * K is consumed in slices of 64 (four K = 16 MMA steps), accumulators live in TMEM (<= 128 columns per CTA, so two
-//     CTAs share an SM and overlap each other's staging / MMA / epilogue);
+//   * K is consumed in slices of 64 (four K = 16 MMA steps), accumulators live in registers (<= 128 columns per CTA:
+//     64 fp32 registers per thread);
 //   * forward products keep six BF16x3 terms (FP32-accurate), gradient products three (2-plane delta, 2^-16).
 // wgrad contracts over ROWS: the same planes, MN-major view (A = dY^T, B = X^T), 8 K-steps per 128-row tile.
 #pragma once
@@ -22,14 +22,14 @@
 namespace gops {
 namespace dense {
 
-constexpr int TM = 128;          // rows per CTA tile (UMMA M)
+constexpr int TM = 128;          // rows per CTA tile (two wgmma M = 64 halves)
 constexpr int KS = 64;           // K slice
 constexpr int NCMAX = 128;       // output columns per CTA
 constexpr int NTH = 256;         // threads per CTA
 
 __host__ __device__ inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
-// columns per CTA / number of column splits for an output width n
-__host__ __device__ inline int nc_of(int n) { const int p = round_up(n, 16); return p < NCMAX ? p : NCMAX; }
+// columns per CTA (a wgmma tile width: 16, 32, 64 or 128) / number of column splits for an output width n
+__host__ __device__ inline int nc_of(int n) { return n <= 16 ? 16 : n <= 32 ? 32 : n <= 64 ? 64 : NCMAX; }
 __host__ __device__ inline int splits_of(int n) { return (round_up(n, 16) + NCMAX - 1) / NCMAX; }
 __host__ __device__ inline int slices_of(int k) { return (k + KS - 1) / KS; }
 // bytes of one packed (split, slice) image: 3 planes x 8 chunks x NC rows x 16 B
@@ -137,34 +137,61 @@ __device__ __forceinline__ void store_tile(const TileRegs& t, unsigned char* pla
   }
 }
 
-// One 128-row x NC-column output tile.  grid = (row tiles, column splits), 256 threads, <= 128 TMEM columns.
+// One 128-row x NC-column output tile.  grid = (row tiles, column splits), 256 threads = two warpgroups, warpgroup w
+// owns rows [64 w, 64 w + 64) of the tile and their NC accumulator columns in registers.
 // GRAD: gradient product (A in two planes, three terms); else forward product (three planes, six terms).
 // K slices are double buffered: while the tensor core works on slice t the CTA converts slice t + 1 into the other
-// operand buffer and its weight image arrives by TMA; MMAs retire in order, so one wait on the last commit ends the loop.
-template <int EPI, bool GRAD>
-__global__ void __launch_bounds__(NTH, 1) dense_gemm_kernel(const __grid_constant__ GemmArgs g) {
-  extern __shared__ __align__(128) unsigned char dsm[];
-  uint64_t* bars = reinterpret_cast<uint64_t*>(dsm);           // [0..1] weights landed (per buffer), [2..3] MMAs retired
-  uint32_t* tslot = reinterpret_cast<uint32_t*>(dsm + 64);
+// operand buffer and its weight image arrives by TMA; a warpgroup keeps at most one slice's wgmma group in flight.
+template <int EPI, int NC, int ACT>
+__device__ __forceinline__ void gemm_epilogue(const GemmArgs& g, const float* acc, long long r0, int split) {
+  const int wgi = threadIdx.x >> 7, t = threadIdx.x & 127;
+#pragma unroll
+  for (int i = 0; i < NC / 2; i += 2) {
+    const long long row = r0 + 64 * wgi + wg::frag_row(t, i);
+    const int n = split * NC + wg::frag_col(t, i);
+    if (row >= g.rows) continue;
+    float v0 = acc[i], v1 = acc[i + 1], d0 = 0.f, d1 = 0.f;
+    if constexpr (EPI == EPI_ACT) {
+      const float b0 = n < g.n ? g.bias[n] : 0.f, b1 = n + 1 < g.n ? g.bias[n + 1] : 0.f;
+      act_fwd_grad_pair_t<ACT>(f32x2::add(f32x2::pk(v0, v1), f32x2::pk(b0, b1)), v0, v1, d0, d1);
+    } else if constexpr (EPI == EPI_LINEAR) {
+      v0 += n < g.n ? g.bias[n] : 0.f;
+      v1 += n + 1 < g.n ? g.bias[n + 1] : 0.f;
+    } else if constexpr (EPI == EPI_MUL) {
+      v0 *= n < g.n ? g.mul[row * g.ldm + n] : 0.f;
+      v1 *= n + 1 < g.n ? g.mul[row * g.ldm + n + 1] : 0.f;
+    }
+    if (n < g.n) g.Y[row * g.ldy + n] = v0;
+    if (n + 1 < g.n) g.Y[row * g.ldy + n + 1] = v1;
+    if constexpr (EPI == EPI_ACT) {
+      if (g.D != nullptr) {
+        if (n < g.n) g.D[row * g.ldd + n] = d0;
+        if (n + 1 < g.n) g.D[row * g.ldd + n + 1] = d1;
+      }
+    }
+  }
+}
+
+template <int EPI, bool GRAD, int NC>
+__device__ __forceinline__ void dense_gemm_body(const GemmArgs& g, unsigned char* dsm) {
+  uint64_t* bars = reinterpret_cast<uint64_t*>(dsm);           // [0..1] weights landed (per buffer)
   constexpr int APL = 8 * TM * 16, NPA = GRAD ? 2 : 3;
-  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-  const int nc = nc_of(g.n), nsl = slices_of(g.k);
-  const size_t img = slice_bytes(nc);
+  const int tid = threadIdx.x, wgi = tid >> 7;
+  const int nsl = slices_of(g.k);
+  const size_t img = slice_bytes(NC);
   unsigned char* Abuf = dsm + 128;
   unsigned char* Bbuf = Abuf + 2 * NPA * APL;
   const int split = blockIdx.y;
   const long long r0 = (long long)blockIdx.x * TM;
-  const uint32_t ncols = nc < 32 ? 32u : (nc <= 64 ? 64u : 128u);
   if (tid == 0) {
-    for (int i = 0; i < 4; ++i) mbar_init(bars + i, 1);
+    mbar_init(bars, 1);
+    mbar_init(bars + 1, 1);
     fence_mbar_init();
   }
-  if (warp == 0) umma::tmem_alloc(tslot, ncols);
-  umma::fence_before_sync();
-  __syncthreads();
-  umma::fence_after_sync();
-  const uint32_t tm = __shfl_sync(0xffffffffu, *tslot, 0);
   const unsigned char* Bsrc = g.Bimg + (size_t)split * nsl * img;
+  float acc[NC / 2];
+#pragma unroll
+  for (int i = 0; i < NC / 2; ++i) acc[i] = 0.f;
   TileRegs regs;
   load_tile(g.A, g.lda, r0, g.rows, 0, g.k, regs);
   for (int t = 0; t < nsl; ++t) {
@@ -172,10 +199,7 @@ __global__ void __launch_bounds__(NTH, 1) dense_gemm_kernel(const __grid_constan
     const uint32_t ph = (uint32_t)(t >> 1) & 1u;
     unsigned char* Ap = Abuf + bf * NPA * APL;
     unsigned char* Bp = Bbuf + (size_t)bf * img;
-    if (t >= 2) {                                   // the MMAs of slice t - 2 read this buffer pair
-      mbar_wait(bars + 2 + bf, ph ^ 1u);
-      umma::fence_after_sync();
-    }
+    __syncthreads();                                // both warpgroups retired slice t - 2, the reader of this buffer pair
     if (tid == 0) {
       fence_proxy_async();
       mbar_expect_tx(bars + bf, (uint32_t)img);
@@ -186,103 +210,61 @@ __global__ void __launch_bounds__(NTH, 1) dense_gemm_kernel(const __grid_constan
     if (t + 1 < nsl) load_tile(g.A, g.lda, r0, g.rows, (t + 1) * KS, g.k, regs);   // next slice's reads are in flight
     fence_proxy_async();
     mbar_wait(bars + bf, ph);
-    umma::fence_before_sync();
     __syncthreads();
-    if (warp == 0) {
-      if (umma::elect_one()) {
-        using namespace tcf;
-        umma::fence_after_sync();
-        const Op A{smem_u32(Ap), (uint32_t)APL, 2048u, 128u, 4096u};
-        const Op B{smem_u32(Bp), (uint32_t)(8 * nc * 16), (uint32_t)(nc * 16), 128u, (uint32_t)(2 * nc * 16)};
-        const uint32_t idesc = idesc_bf16(128, nc, false, false);
-        const uint64_t ka = A.kadv >> 4, kb = B.kadv >> 4;
-        const uint64_t a0 = dsc(A, 0), a1 = dsc(A, 1), b0 = dsc(B, 0), b1 = dsc(B, 1), b2 = dsc(B, 2);
-        uint32_t first = t == 0 ? 0u : 1u;
-        if constexpr (!GRAD) {
-          const uint64_t a2 = dsc(A, 2);
+    {
+      using namespace tcf;
+      const Op A{smem_u32(Ap) + 1024u * wgi, (uint32_t)APL, 2048u, 128u, 4096u};     // this warpgroup's 64 rows
+      const Op B{smem_u32(Bp), (uint32_t)(8 * NC * 16), (uint32_t)(NC * 16), 128u, (uint32_t)(2 * NC * 16)};
+      const uint64_t ka = A.kadv >> 4, kb = B.kadv >> 4;
+      const uint64_t a0 = dsc(A, 0), a1 = dsc(A, 1), b0 = dsc(B, 0), b1 = dsc(B, 1), b2 = dsc(B, 2);
+      uint32_t first = t == 0 ? 0u : 1u;
+      wg::fence();
+      if constexpr (!GRAD) {
+        const uint64_t a2 = dsc(A, 2);
 #pragma unroll
-          for (int ks = 0; ks < 4; ++ks) { mma_bf16(tm, a2 + ks * ka, b0 + ks * kb, idesc, first); first = 1u; }
+        for (int ks = 0; ks < 4; ++ks) { wg::mma_bf16<NC, 0, 0>(acc, a2 + ks * ka, b0 + ks * kb, first); first = 1u; }
 #pragma unroll
-          for (int ks = 0; ks < 4; ++ks) mma_bf16(tm, a0 + ks * ka, b2 + ks * kb, idesc, 1u);
+        for (int ks = 0; ks < 4; ++ks) wg::mma_bf16<NC, 0, 0>(acc, a0 + ks * ka, b2 + ks * kb, 1u);
 #pragma unroll
-          for (int ks = 0; ks < 4; ++ks) mma_bf16(tm, a1 + ks * ka, b1 + ks * kb, idesc, 1u);
-        }
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) { mma_bf16(tm, a1 + ks * ka, b0 + ks * kb, idesc, first); first = 1u; }
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) mma_bf16(tm, a0 + ks * ka, b1 + ks * kb, idesc, 1u);
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) mma_bf16(tm, a0 + ks * ka, b0 + ks * kb, idesc, 1u);
-        umma::commit(bars + 2 + bf);
+        for (int ks = 0; ks < 4; ++ks) wg::mma_bf16<NC, 0, 0>(acc, a1 + ks * ka, b1 + ks * kb, 1u);
       }
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) { wg::mma_bf16<NC, 0, 0>(acc, a1 + ks * ka, b0 + ks * kb, first); first = 1u; }
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) wg::mma_bf16<NC, 0, 0>(acc, a0 + ks * ka, b1 + ks * kb, 1u);
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) wg::mma_bf16<NC, 0, 0>(acc, a0 + ks * ka, b0 + ks * kb, 1u);
+      wg::commit();
     }
+    wg::wait<1>();
   }
-  {  // MMAs retire in order: the last slice's commit covers all of them
-    const int tl = nsl - 1;
-    mbar_wait(bars + 2 + (tl & 1), (uint32_t)(tl >> 1) & 1u);
-    umma::fence_after_sync();
+  wg::wait<0>();
+  wg::reg_fence<NC / 2>(acc);
+  if constexpr (EPI == EPI_ACT) {
+#define GOPS_DENSE_EPI(A) gemm_epilogue<EPI, NC, A>(g, acc, r0, split)
+    GOPS_ACT_SWITCH(g.act, GOPS_DENSE_EPI)
+#undef GOPS_DENSE_EPI
+  } else {
+    gemm_epilogue<EPI, NC, GOPS_ACT_LINEAR>(g, acc, r0, split);
   }
-  // ---- epilogue: thread = (row, half of the tile's columns), 16 columns per pass
-  {
-    const int q = warp & 3, half = warp >> 2, lane = tid & 31;
-    const long long row = r0 + 32 * q + lane;
-    const uint32_t tl = tm + ((uint32_t)(32 * q) << 16);
-    const int blocks = nc / 16, per = (blocks + 1) / 2;
-    for (int b = half * per; b < blocks && b < (half + 1) * per; ++b) {
-      float v[16], d[16];
-      umma::tmem_ld16(tl + 16 * b, v);
-      const int n0 = split * nc + 16 * b;
-      if (row < g.rows) {
-        if constexpr (EPI == EPI_ACT) {
-#define GOPS_DENSE_ACT(A)                                                                     \
-  _Pragma("unroll") for (int e = 0; e < 16; e += 2) {                                         \
-    const float b0 = n0 + e < g.n ? g.bias[n0 + e] : 0.f, b1 = n0 + e + 1 < g.n ? g.bias[n0 + e + 1] : 0.f; \
-    act_fwd_grad_pair_t<A>(f32x2::add(f32x2::pk(v[e], v[e + 1]), f32x2::pk(b0, b1)), v[e], v[e + 1], d[e], d[e + 1]); \
+}
+
+template <int EPI, bool GRAD>
+__global__ void __launch_bounds__(NTH, 1) dense_gemm_kernel(const __grid_constant__ GemmArgs g) {
+  extern __shared__ __align__(128) unsigned char dsm[];
+  switch (nc_of(g.n)) {
+    case 16: dense_gemm_body<EPI, GRAD, 16>(g, dsm); break;
+    case 32: dense_gemm_body<EPI, GRAD, 32>(g, dsm); break;
+    case 64: dense_gemm_body<EPI, GRAD, 64>(g, dsm); break;
+    default: dense_gemm_body<EPI, GRAD, 128>(g, dsm); break;
   }
-          GOPS_ACT_SWITCH(g.act, GOPS_DENSE_ACT)
-#undef GOPS_DENSE_ACT
-        } else if constexpr (EPI == EPI_LINEAR) {
-#pragma unroll
-          for (int e = 0; e < 16; ++e) v[e] += (n0 + e < g.n ? g.bias[n0 + e] : 0.f);
-        } else if constexpr (EPI == EPI_MUL) {
-#pragma unroll
-          for (int e = 0; e < 16; ++e) v[e] *= (n0 + e < g.n ? g.mul[row * g.ldm + n0 + e] : 0.f);
-        }
-        if (n0 + 16 <= g.n && (g.ldy & 3) == 0) {
-#pragma unroll
-          for (int e4 = 0; e4 < 4; ++e4)
-            *reinterpret_cast<float4*>(g.Y + row * g.ldy + n0 + 4 * e4) = make_float4(v[4 * e4], v[4 * e4 + 1], v[4 * e4 + 2], v[4 * e4 + 3]);
-        } else {
-#pragma unroll
-          for (int e = 0; e < 16; ++e)
-            if (n0 + e < g.n) g.Y[row * g.ldy + n0 + e] = v[e];
-        }
-        if constexpr (EPI == EPI_ACT) {
-          if (g.D != nullptr) {
-            if (n0 + 16 <= g.n && (g.ldd & 3) == 0) {
-#pragma unroll
-              for (int e4 = 0; e4 < 4; ++e4)
-                *reinterpret_cast<float4*>(g.D + row * g.ldd + n0 + 4 * e4) = make_float4(d[4 * e4], d[4 * e4 + 1], d[4 * e4 + 2], d[4 * e4 + 3]);
-            } else {
-#pragma unroll
-              for (int e = 0; e < 16; ++e)
-                if (n0 + e < g.n) g.D[row * g.ldd + n0 + e] = d[e];
-            }
-          }
-        }
-      }
-    }
-  }
-  umma::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) umma::tmem_dealloc(tm, ncols);
 }
 
 inline size_t gemm_smem(int n, bool grad) { return 128 + 2 * ((size_t)(grad ? 2 : 3) * 8 * TM * 16 + slice_bytes(nc_of(n))); }
 
 // dW partial of one (128 output features, <= 128 input features) block over a chunk of the rows:
 // grid = (n blocks * k blocks, row chunks).  A = dY^T (2 planes), B = X^T (2 planes), contraction over rows: the planes are
-// the K-major images of the [row][feature] tiles, read MN-major (umma.cuh), three terms a1b0 + a0b1 + a0b0.
+// the K-major images of the [row][feature] tiles, read MN-major (wgmma.cuh), three terms a1b0 + a0b1 + a0b0.
 // The rows may be spread over `nslots` equally shaped slabs (the per-step slots of a rollout): slab s of dY starts at
 // dY + s * sy * ldy, of X at X + s * sx * ldx, each with `rows` valid rows -> ONE contraction over all steps and samples.
 struct WgradArgs {
@@ -291,95 +273,78 @@ struct WgradArgs {
   int tiles_per_chunk;
   int nslots; long long sy, sx;
 };
-__global__ void __launch_bounds__(NTH, 1) dense_wgrad_kernel(const __grid_constant__ WgradArgs g) {
-  extern __shared__ __align__(128) unsigned char dsm[];
-  uint64_t* bars = reinterpret_cast<uint64_t*>(dsm);
-  uint32_t* tslot = reinterpret_cast<uint32_t*>(dsm + 32);
+template <int KW>
+__device__ __forceinline__ void dense_wgrad_body(const WgradArgs& g, unsigned char* dsm, int n0, int k0) {
   constexpr int PL = 16 * TM * 16;                            // one plane: 128 features = 16 chunks x 128 rows x 16 B
   unsigned char* Yp = dsm + 128;
   unsigned char* Xp = Yp + 2 * PL;
-  const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-  const int kb = (g.k + 127) / 128, nb_i = blockIdx.x / kb, kb_i = blockIdx.x % kb;
-  const int n0 = nb_i * 128, k0 = kb_i * 128;
-  const int kw = round_up((g.k - k0) < 128 ? (g.k - k0) : 128, 16);        // MMA N extent
-  const uint32_t ncols = kw <= 32 ? 32u : (kw <= 64 ? 64u : 128u);
-  if (tid == 0) {
-    mbar_init(bars, 1);
-    fence_mbar_init();
-  }
-  if (warp == 0) umma::tmem_alloc(tslot, ncols);
-  umma::fence_before_sync();
-  __syncthreads();
-  umma::fence_after_sync();
-  const uint32_t tm = __shfl_sync(0xffffffffu, *tslot, 0);
+  const int tid = threadIdx.x, wgi = tid >> 7, tw = tid & 127;
   const long long t0 = (long long)blockIdx.y * g.tiles_per_chunk;
   const long long tps = (g.rows + TM - 1) / TM, ttot = tps * g.nslots;      // tiles per slab, tiles in total
-  uint32_t ph = 0, first = 0u;
-  TileRegs ra, rb, rc, rd;
-  auto load4 = [&](long long tt) {
+  uint32_t first = 0u;
+  float acc[KW / 2];
+#pragma unroll
+  for (int i = 0; i < KW / 2; ++i) acc[i] = 0.f;
+  // tile q of row tile tt: q = 0 / 1 the dY columns [n0, n0 + 64) / [n0 + 64, n0 + 128), q = 2 / 3 the X columns
+  auto load_q = [&](long long tt, int q, TileRegs& r) {
     const long long slab = tt / tps, r0 = (tt - slab * tps) * TM;
-    const float* dYs = g.dY + slab * g.sy * g.ldy;
-    const float* Xs = g.X + slab * g.sx * g.ldx;
-    load_tile(dYs, g.ldy, r0, g.rows, n0, g.n, ra);
-    load_tile(dYs, g.ldy, r0, g.rows, n0 + 64, g.n, rb);
-    load_tile(Xs, g.ldx, r0, g.rows, k0, g.k, rc);
-    if (kw > 64) load_tile(Xs, g.ldx, r0, g.rows, k0 + 64, g.k, rd);
+    if (q < 2) load_tile(g.dY + slab * g.sy * g.ldy, g.ldy, r0, g.rows, n0 + 64 * q, g.n, r);
+    else load_tile(g.X + slab * g.sx * g.ldx, g.ldx, r0, g.rows, k0 + 64 * (q - 2), g.k, r);
   };
-  if (t0 < ttot) load4(t0);
+  auto store_q = [&](int q, const TileRegs& r) { store_tile<2>(r, (q < 2 ? Yp : Xp) + (q & 1) * 8 * TM * 16, PL); };
+  constexpr int NQ = KW > 64 ? 4 : 3;
+  // each tile is loaded and stored in turn (no prefetch across the MMAs: three or four tiles held in registers next to
+  // up to 64 accumulator registers per thread spill)
+  TileRegs rt;
   for (int t = 0; t < g.tiles_per_chunk; ++t) {
     const long long tt = t0 + t;
     if (tt >= ttot) break;
-    store_tile<2>(ra, Yp, PL);
-    store_tile<2>(rb, Yp + 8 * TM * 16, PL);
-    store_tile<2>(rc, Xp, PL);
-    if (kw > 64) store_tile<2>(rd, Xp + 8 * TM * 16, PL);
+#pragma unroll
+    for (int q = 0; q < NQ; ++q) {
+      load_q(tt, q, rt);
+      store_q(q, rt);
+    }
     fence_proxy_async();
-    umma::fence_before_sync();
     __syncthreads();
-    if (warp == 0) {
-      if (umma::elect_one()) {
-        using namespace tcf;
-        umma::fence_after_sync();
-        const Op A = mn_act(Yp, PL), B = mn_act(Xp, PL);
-        const uint32_t idesc = idesc_bf16(128, kw, true, true);
-        const uint64_t ka = A.kadv >> 4, kbv = B.kadv >> 4;
-        const uint64_t a0 = dsc(A, 0), a1 = dsc(A, 1), b0 = dsc(B, 0), b1 = dsc(B, 1);
+    {
+      using namespace tcf;
+      // M = this warpgroup's 64 output features (chunks 8 wgi ..), N = input features, K = the tile's 128 rows
+      const Op A{smem_u32(Yp) + (uint32_t)(8 * TM * 16) * wgi, (uint32_t)PL, 128u, 2048u, 256u};
+      const Op B{smem_u32(Xp), (uint32_t)PL, 128u, 2048u, 256u};
+      const uint64_t ka = A.kadv >> 4, kbv = B.kadv >> 4;
+      const uint64_t a0 = dsc(A, 0), a1 = dsc(A, 1), b0 = dsc(B, 0), b1 = dsc(B, 1);
+      wg::fence();
 #pragma unroll
-        for (int ks = 0; ks < 8; ++ks) { mma_bf16(tm, a1 + ks * ka, b0 + ks * kbv, idesc, first); first = 1u; }
+      for (int ks = 0; ks < 8; ++ks) { wg::mma_bf16<KW, 1, 1>(acc, a1 + ks * ka, b0 + ks * kbv, first); first = 1u; }
 #pragma unroll
-        for (int ks = 0; ks < 8; ++ks) mma_bf16(tm, a0 + ks * ka, b1 + ks * kbv, idesc, 1u);
+      for (int ks = 0; ks < 8; ++ks) wg::mma_bf16<KW, 1, 1>(acc, a0 + ks * ka, b1 + ks * kbv, 1u);
 #pragma unroll
-        for (int ks = 0; ks < 8; ++ks) mma_bf16(tm, a0 + ks * ka, b0 + ks * kbv, idesc, 1u);
-        umma::commit(bars);
-      }
+      for (int ks = 0; ks < 8; ++ks) wg::mma_bf16<KW, 1, 1>(acc, a0 + ks * ka, b0 + ks * kbv, 1u);
+      wg::commit();
     }
-    first = 1u;
-    if (t + 1 < g.tiles_per_chunk && tt + 1 < ttot) load4(tt + 1);      // next tile's reads fly during the MMAs
-    mbar_wait(bars, ph);
-    umma::fence_after_sync();
-    ph ^= 1u;
+    wg::wait<0>();
+    __syncthreads();                                                     // both warpgroups are done with the planes
   }
-  {  // epilogue: lane = output feature, columns = input features
-    const int q = warp & 3, half = warp >> 2, lane = tid & 31;
-    const int n = n0 + 32 * q + lane;
-    const uint32_t tl = tm + ((uint32_t)(32 * q) << 16);
-    float* out = g.partial + (size_t)blockIdx.y * g.n * g.k;
-    const int blocks = kw / 16, per = (blocks + 1) / 2;
-    for (int b = half * per; b < blocks && b < (half + 1) * per; ++b) {
-      float v[16];
-      umma::tmem_ld16(tl + 16 * b, v);
-      if (n < g.n) {
+  wg::reg_fence<KW / 2>(acc);
+  // epilogue: fragment row = output feature, column = input feature
+  float* out = g.partial + (size_t)blockIdx.y * g.n * g.k;
 #pragma unroll
-        for (int e = 0; e < 16; ++e) {
-          const int k = k0 + 16 * b + e;
-          if (k < g.k) out[(size_t)n * g.k + k] = first ? v[e] : 0.f;     // a chunk past the last row writes zeros
-        }
-      }
-    }
+  for (int i = 0; i < KW / 2; ++i) {
+    const int n = n0 + 64 * wgi + wg::frag_row(tw, i), k = k0 + wg::frag_col(tw, i);
+    if (n < g.n && k < g.k) out[(size_t)n * g.k + k] = first ? acc[i] : 0.f;     // a chunk past the last row writes zeros
   }
-  umma::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) umma::tmem_dealloc(tm, ncols);
+}
+
+// dW partial of one (128 output features, <= 128 input features) block over a chunk of the rows
+__global__ void __launch_bounds__(NTH, 1) dense_wgrad_kernel(const __grid_constant__ WgradArgs g) {
+  extern __shared__ __align__(128) unsigned char dsm[];
+  const int kb = (g.k + 127) / 128, nb_i = blockIdx.x / kb, kb_i = blockIdx.x % kb;
+  const int n0 = nb_i * 128, k0 = kb_i * 128;
+  const int kw = (g.k - k0) < 128 ? (g.k - k0) : 128;                   // input features of this block
+  if (kw <= 16) dense_wgrad_body<16>(g, dsm, n0, k0);
+  else if (kw <= 32) dense_wgrad_body<32>(g, dsm, n0, k0);
+  else if (kw <= 64) dense_wgrad_body<64>(g, dsm, n0, k0);
+  else dense_wgrad_body<128>(g, dsm, n0, k0);
 }
 inline size_t wgrad_smem() { return 128 + (size_t)4 * 16 * TM * 16; }
 

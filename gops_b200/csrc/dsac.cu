@@ -2,7 +2,7 @@
 // evaluations -- reparameterised tanh-Gaussian action sampling with its log-density (act_distribution_type.py:18-50),
 // the distributional critic loss with the clipped TD target (dsac.py:219-262), the actor loss (dsac.py:264-270) -- each
 // with its hand-derived gradient towards the network outputs.  The network evaluations themselves run on the
-// layer-wise tcgen05 MLP (dense_tc.cu).  All reductions are fixed-order (deterministic).
+// layer-wise wgmma MLP (dense_tc.cu).  All reductions are fixed-order (deterministic).
 #include "gops_b200.h"
 
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// libgops_b200.so: C ABI (include/gops_b200.h) over the fused sm_100a rollout kernels.
+// libgops_b200.so: C ABI (include/gops_b200.h) over the fused sm_90a rollout kernels.
 #include "gops_b200.h"
 
 #include <cuda_runtime.h>
@@ -166,7 +166,7 @@ void launch_veh_step_detour(const KParams& p, const float* action, float* next_o
                             float* next_state, cudaStream_t st);
 void lw_launch_scalars_detour(const KParams& p, const float* vacc, const float* cacc, const float* dn_last, float* scalars,
                               cudaStream_t st);
-RolloutFn rollout_fn_tc2_idp(int alg, int hact);  // pipelined tcgen05 kernel: two independent 128-thread groups per CTA (rollout_tc2.cuh)
+RolloutFn rollout_fn_tc2_idp(int alg, int hact);  // wgmma rollout kernel (rollout_tc2.cuh)
 RolloutFn rollout_fn_tc2_lq(int alg, int hact);
 }  // namespace gops
 
@@ -221,9 +221,9 @@ struct gops_b200_plan {
   size_t ext_ref_floats = 0;
   float* xbuf = nullptr;
   size_t xbuf_floats = 0;
-  float* blob_tc = nullptr;     // tcgen05 inference path: chunk-major hi / lo weight planes
+  float* blob_tc = nullptr;     // wgmma inference path: chunk-major hi / lo weight planes
   int blob_tc_floats = 0;
-  // full tcgen05 rollout kernel (BF16x3): NetL with the bf16-plane blob offsets, packed blobs
+  // wgmma rollout kernel (BF16x3): NetL with the bf16-plane blob offsets, packed blobs
   bool tc_ok = false;
   NetL pol_tcf, val_tcf;
   int w_floats_tcf = 0;
@@ -234,7 +234,7 @@ struct gops_b200_plan {
   bool timing = false;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   int path = GOPS_PATH_AUTO, last_path = 0;
-  // layer-wise tcgen05 path of the wide nets (lw_rollout.cuh + dense_tc.cu)
+  // layer-wise wgmma path of the wide nets (lw_rollout.cuh + dense_tc.cu)
   gops_b200_mlpnet* lw_net = nullptr;
   long long lw_cap = 0;
   float *lw_S = nullptr, *lw_Dn = nullptr, *lw_X = nullptr, *lw_Z = nullptr, *lw_Zb = nullptr, *lw_lam = nullptr,
@@ -265,8 +265,8 @@ size_t infer_smem_bytes(const KParams& kp, int S, int NT) {
   return sizeof(float) * (size_t)(4 + kp.w_floats + kp.inp_max * XS + 2 * HID * SP + 8 * XS);
 }
 
-// NetL of the full tcgen05 path: blob = 3 bf16 planes of W1 ([2][64][8]) and W2 ([8][64][8]), then fp32 W3, b1, b2, b3
-// (offsets in floats); shared-memory accumulators only for W3 / b3 (the rest accumulates in TMEM)
+// NetL of the wgmma rollout path: blob = 3 bf16 planes of W1 ([2][64][8]) and W2 ([8][64][8]), then fp32 W3, b1, b2, b3
+// (offsets in floats); shared-memory accumulators only for W3 / b3 (the rest is added into the FP32 partial every step)
 void make_net_tcf(const NetL& base, NetL& L) {
   L = base;
   int o = 0;
@@ -284,7 +284,7 @@ void make_net_tcf(const NetL& base, NetL& L) {
   L.nacc = L.out * 64 + L.out;
 }
 // Path of a launch: the plan option (gops_b200_plan_set_path), overridden by GOPS_B200_ROLLOUT=tc|mma; AUTO takes the
-// tcgen05 kernel wherever it is built for the plan (64-wide nets, <= 16 inputs, state == obs models)
+// wgmma kernel wherever it is built for the plan (64-wide nets, <= 16 inputs, state == obs models)
 bool rollout_use_tc(const gops_b200_plan* pl, long long batch) {
   if (!pl->tc_ok) return false;
   int path = pl->path;
@@ -293,8 +293,10 @@ bool rollout_use_tc(const gops_b200_plan* pl, long long batch) {
   if (e && !strcmp(e, "tc")) path = GOPS_PATH_TC;
   if (path == GOPS_PATH_MMA) return false;
   if (path == GOPS_PATH_TC) return true;
-  // the pipelined kernel schedules single 128-sample sub-tiles; below ~2^14 samples (fewer sub-tiles than SM slots) the
-  // mma.sync kernel with its 32-sample tiles spreads the batch over more SMs and finishes first (bench.py configs, C5 sweep)
+  // the wgmma kernel schedules single 128-sample sub-tiles; below ~2^14 samples (fewer sub-tiles than SMs) the mma.sync
+  // kernel with its 32-sample tiles spreads the batch over more SMs and finishes first.  Measured on one H100 80GB HBM3
+  // (700 W), ms per update mma / wgmma: FHADP idpendulum H = 30  2^13 0.74 / 0.78, 2^14 1.20 / 0.78, 2^18 11.8 / 10.4;
+  // INFADP lq s4a2 PEV + PIM  2^12 0.66 / 0.69, 2^14 0.86 / 0.71.
   return batch >= 16384;
 }
 __global__ void pack_params_tcf_kernel(const float* __restrict__ flat, NetL L, float* __restrict__ blob) {
@@ -396,7 +398,7 @@ int launch_pack(const float* flat, const NetL& L, int hid, float* blob, cudaStre
   return 0;
 }
 
-// Wide nets (hidden 256), FHADP: the layer-wise tcgen05 path.  AUTO takes it wherever it is built; MMA keeps the fused
+// Wide nets (hidden 256), FHADP: the layer-wise wgmma path.  AUTO takes it wherever it is built; MMA keeps the fused
 // FP32-FFMA kernel (A/B baseline).
 bool rollout_use_layerwise(const gops_b200_plan* pl, int alg) {
   if (pl->desc.open_loop || pl->desc.veh_detour) return alg == ALG_FHADP;
@@ -619,7 +621,7 @@ int launch_rollout(gops_b200_plan* pl, const gops_b200_batch* b, int alg, cudaSt
     const bool v1 = false;
     const int hact = (alg == ALG_FHADP || pl->pol_tcf.hact == pl->val_tcf.hact) ? pl->pol_tcf.hact : -1;
     RolloutFn fn = rollout_fn_tc2(pl->desc.model, alg, hact);
-    if (!fn) return fail("tcgen05 rollout kernel not built for this env model");
+    if (!fn) return fail("wgmma rollout kernel not built for this env model");
     const int S = 128, NT = v1 ? 512 : tc2::NT2;
     KParams k2 = kp;
     k2.pol = pl->pol_tcf;
@@ -640,13 +642,13 @@ int launch_rollout(gops_b200_plan* pl, const gops_b200_batch* b, int alg, cudaSt
     kp.part_stride = k2.part_stride;
     k2.dw_floats = round4(upd.nacc);
     const size_t smem = tc2::smem_bytes(k2.w_floats);
-    if (smem > (size_t)pl->max_smem) return fail("tcgen05 rollout kernel does not fit in shared memory");
+    if (smem > (size_t)pl->max_smem) return fail("wgmma rollout kernel does not fit in shared memory");
     bool& attr = v1 ? pl->tc_attr_set[alg] : pl->tc2_attr_set[alg];
     if (!attr) {
       CUDA_OK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, pl->max_smem));
       attr = true;
     }
-    const long long slots = pl->sm_count;          // one CTA per SM (all 512 TMEM columns)
+    const long long slots = pl->sm_count;          // one CTA per SM (shared memory)
     const long long subtiles = (b->batch + S - 1) / S;
     const int rows = v1 ? 1 : tc2::NG;             // gradient partial rows (= independent groups) per CTA
     const long long want = (subtiles + rows - 1) / rows;
@@ -656,31 +658,10 @@ int launch_rollout(gops_b200_plan* pl, const gops_b200_batch* b, int alg, cudaSt
     k2.ext_ref = pl->ext_ref;
     k2.xbuf = pl->xbuf;
     k2.partial = pl->partial;
-    const char* tlf = getenv("GOPS_B200_TIMELINE");      // development aid (build with -DGOPS_TC2_TIMELINE): clock64 stamps
-    long long* dbg = nullptr;
-    if (tlf && !v1) {
-      CUDA_OK(cudaMalloc(&dbg, 8192 * sizeof(long long)));
-      CUDA_OK(cudaMemset(dbg, 0, 8192 * sizeof(long long)));
-    }
-    k2.dbg = dbg;
     if (pl->timing) CUDA_OK(cudaEventRecord(pl->ev0, st));
     fn<<<grid, NT, smem, st>>>(k2);
     ++g_launches;
     CUDA_OK_L(cudaGetLastError(), "launch#2-tc");
-    if (dbg) {
-      std::vector<long long> h(8192);
-      CUDA_OK(cudaStreamSynchronize(st));
-      CUDA_OK(cudaMemcpy(h.data(), dbg, h.size() * sizeof(long long), cudaMemcpyDeviceToHost));
-      cudaFree(dbg);
-      if (FILE* f = fopen(tlf, "w")) {
-        for (int who = 0; who < 2; ++who) {
-          const long long n = h[who * 4096 + 4095];
-          for (long long i = 0; i < n && i < 4000; ++i)
-            fprintf(f, "%d %lld %lld\n", who, h[who * 4096 + i] & 255, h[who * 4096 + i] >> 8);
-        }
-        fclose(f);
-      }
-    }
     if (pl->timing) CUDA_OK(cudaEventRecord(pl->ev1, st));
     pl->last_grid = grid; pl->last_S = S; pl->last_NT = NT; pl->last_smem = smem; pl->last_path = GOPS_PATH_TC;
     if (alg != ALG_TRACE) {
@@ -892,7 +873,7 @@ int gops_b200_plan_create(const gops_b200_plan_desc* d, gops_b200_plan** out) {
   cudaDeviceProp prop;
   if (e == cudaSuccess) e = cudaGetDeviceProperties(&prop, pl->device);
   if (e != cudaSuccess) { delete pl; return fail(std::string("no CUDA device: ") + cudaGetErrorString(e)); }
-  if (prop.major < 10) { delete pl; return fail("gops_b200 requires an sm_100a (B200) device"); }
+  if (prop.major != 9 || prop.minor != 0) { delete pl; return fail("gops_b200 is built for sm_90a and needs an H100-class (sm_90) device"); }
   pl->sm_count = prop.multiProcessorCount;
   pl->max_smem = (int)prop.sharedMemPerBlockOptin;
 
@@ -923,7 +904,7 @@ int gops_b200_plan_create(const gops_b200_plan_desc* d, gops_b200_plan** out) {
     kp.osc = pl->osc;
     kp.osh = pl->osc + od;
   }
-  // full tcgen05 rollout kernel: 64-wide nets whose inputs fit one 16-wide K block, state == obs models
+  // wgmma rollout kernel: 64-wide nets whose inputs fit one 16-wide K block, state == obs models
   if (kp.hid == 64 && kp.pol.in <= tcf::K1 && (!infadp || kp.val.in <= tcf::K1) && rollout_fn_tc2(d->model, d->alg)) {
     make_net_tcf(kp.pol, pl->pol_tcf);
     if (infadp) make_net_tcf(kp.val, pl->val_tcf); else pl->val_tcf = pl->pol_tcf;
@@ -932,7 +913,7 @@ int gops_b200_plan_create(const gops_b200_plan_desc* d, gops_b200_plan** out) {
     if (cudaMalloc(&pl->blob_pol_tcf, nb) != cudaSuccess || cudaMalloc(&pl->blob_val_tcf, nb) != cudaSuccess ||
         cudaMalloc(&pl->blob_vtg_tcf, nb) != cudaSuccess) {
       gops_b200_plan_destroy(pl);
-      return fail("cudaMalloc failed for plan scratch (tcgen05 blobs)");
+      return fail("cudaMalloc failed for plan scratch (wgmma rollout blobs)");
     }
     cudaMemset(pl->blob_pol_tcf, 0, nb); cudaMemset(pl->blob_val_tcf, 0, nb); cudaMemset(pl->blob_vtg_tcf, 0, nb);
     pl->tc_ok = true;
@@ -978,7 +959,7 @@ int gops_b200_plan_set_path(gops_b200_plan* pl, int path) {
   if (!pl) return fail("null plan");
   if (path != GOPS_PATH_AUTO && path != GOPS_PATH_MMA && path != GOPS_PATH_TC) return fail("unknown kernel path");
   if (path == GOPS_PATH_TC && !pl->tc_ok && !(pl->kp.hid > 64 && pl->desc.alg == GOPS_ALG_FHADP && lw_fn(pl->desc.model, 0)))
-    return fail("the tcgen05 rollout kernel is not built for this plan (needs 64-wide nets, <= 16 inputs, idpendulum / lq)");
+    return fail("the wgmma rollout kernel is not built for this plan (needs 64-wide nets, <= 16 inputs, idpendulum / lq)");
   pl->path = path;
   return 0;
 }
@@ -1024,10 +1005,11 @@ int gops_b200_plan_destroy(gops_b200_plan* pl) {
                          "blob_pol_tcf", "blob_val_tcf", "blob_vtg_tcf"};
   if (getenv("GOPS_B200_DEBUG")) {
     fprintf(stderr, "[gops_b200] destroy plan %p alg %d model %d:", (void*)pl, pl->desc.alg, pl->desc.model);
-    for (int i = 0; i < 13; ++i) fprintf(stderr, " %s=%p", names[i], ptrs[i]);
+    for (size_t i = 0; i < sizeof(ptrs) / sizeof(ptrs[0]); ++i) fprintf(stderr, " %s=%p", names[i], ptrs[i]);
     fprintf(stderr, "\n");
   }
-  for (int i = 0; i < 13; ++i) {
+  static_assert(sizeof(ptrs) / sizeof(ptrs[0]) == sizeof(names) / sizeof(names[0]), "one name per buffer");
+  for (size_t i = 0; i < sizeof(ptrs) / sizeof(ptrs[0]); ++i) {
     const cudaError_t e = cudaFree(ptrs[i]);
     if (e != cudaSuccess) {
       (void)cudaGetLastError();
@@ -1094,12 +1076,12 @@ int gops_b200_rollout_trace(gops_b200_plan* pl, const gops_b200_batch* b, const 
   return launch_rollout(pl, b, ALG_TRACE, st, nullptr, nullptr);
 }
 
-// tcgen05 / TMEM inference (mlp_tc.cuh).  GOPS_B200_INFER=tc|mma forces one of the two 64-wide paths.
+// wgmma inference (mlp_tc.cuh).  GOPS_B200_INFER=tc|mma forces one of the two 64-wide paths.
 static bool infer_use_tc(const gops_b200_plan* pl, int64_t batch, int use_val) {
   if (pl->kp.hid != 64) return false;
   const char* e = getenv("GOPS_B200_INFER");
   if (e && !strcmp(e, "mma")) return false;
-  // the tcgen05 inference kernel keeps the input planes in shared memory: wide inputs stay on the mma.sync kernel
+  // the wgmma inference kernel keeps the input planes in shared memory: wide inputs stay on the mma.sync kernel
   // whatever the batch size is (no batch-dependent failure)
   const NetL& L = use_val ? pl->kp.val : pl->kp.pol;
   TcNet T;
@@ -1131,7 +1113,7 @@ static int infer_tc(gops_b200_plan* pl, const float* params, const NetL& L, cons
   for (int j = 0; j < MAXA; ++j) { T.half[j] = pl->kp.pol_half[j]; T.mid[j] = pl->kp.pol_mid[j]; }
   const int wgs = tc_infer_smem_bytes(T, 2) <= (size_t)pl->max_smem ? 2 : 1;
   const size_t smem = tc_infer_smem_bytes(T, wgs);
-  if (smem > (size_t)pl->max_smem) return fail("tcgen05 inference: input width does not fit in shared memory");
+  if (smem > (size_t)pl->max_smem) return fail("wgmma inference: input width does not fit in shared memory");
   if (pl->blob_tc_floats < T.blob) {
     if (pl->blob_tc) cudaFree(pl->blob_tc);
     pl->blob_tc = nullptr; pl->blob_tc_floats = 0;

@@ -11,7 +11,7 @@ namespace gops {
 // HD = 256 (WG): they do not fit (519 KB of weights) -> weights are read from the packed blob in global memory
 // (L2 resident, generic loads), gradients accumulate directly in this CTA's global partial, X is a per-CTA global
 // scratch; only the activation tiles stay in shared memory.
-// (The tcgen05 / TMEM rollout kernel is rollout_tc2.cuh; this template is the mma.sync / FFMA family.)
+// (The wgmma rollout kernel is rollout_tc2.cuh; this template is the mma.sync / FFMA family.)
 template <class M, int HD, int S, int NT, int ALG>
 __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ KParams p) {
   constexpr int SP = S + 4, XS = NT + 4, NS = M::NS, HID = HD;

@@ -26,7 +26,7 @@ RolloutFn rollout_fn_lq(int hid, int cfg, int alg) {
     default: return pick<ALG_TRACE>(hid, cfg);
   }
 }
-RolloutFn rollout_fn_tc2_lq(int alg, int hact) {   // pipelined tcgen05 kernel (two independent groups per CTA)
+RolloutFn rollout_fn_tc2_lq(int alg, int hact) {   // wgmma rollout kernel (rollout_tc2.cuh)
   if (hact == GOPS_ACT_GELU) {                       // activation fixed at compile time (rollout_tc2.cuh, GOPS_TC2_ACT_SWITCH)
     switch (alg) {
       case ALG_FHADP: return rollout_tc2_kernel<ModelLq, ALG_FHADP, GOPS_ACT_GELU>;

@@ -1,11 +1,11 @@
 // Layer-wise FHADP rollout for nets that do not fit the fused kernels (hidden width 256): the horizon unroll of
-// gops/algorithm/fhadp.py:113-125 as per-step kernels around the tcgen05 dense layers of dense_tc.cuh.
+// gops/algorithm/fhadp.py:113-125 as per-step kernels around the wgmma dense layers of dense_tc.cuh.
 //
-//   forward step k :  policy MLP on X_k (3 tcgen05 GEMMs, activations kept in slot k)  ->  z_k
+//   forward step k :  policy MLP on X_k (3 wgmma GEMMs, activations kept in slot k)  ->  z_k
 //                     lw_step_kernel: tanh squash / wrapper chain / env-model step -> state_{k+1}, done_{k+1}, X_{k+1}, reward
 //   reverse step k :  lw_reverse_kernel: finish lambda_{k+1} with the observation adjoint of step k + 1's input
 //                     gradient, then the hand-derived adjoint of step k  ->  zbar_k, lambda_k (partial)
-//                     policy MLP backward of slot k (tcgen05 dgrad GEMMs; deltas kept)  ->  dX_k
+//                     policy MLP backward of slot k (wgmma dgrad GEMMs; deltas kept)  ->  dX_k
 //   weight gradients: ONE contraction per layer over all H x B rows (gops_b200_mlpnet_wgrad_slots).
 // Same per-sample arithmetic as the fused kernels (models.cuh / models_veh.cuh device functions), one thread per sample;
 // states live in HBM between the steps: 0.5 GB of activations per update for C3 (8192 x 60 x [256 + 256 + 248] fp32 x2),

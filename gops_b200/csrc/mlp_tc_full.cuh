@@ -1,55 +1,28 @@
-// BF16x3 tcgen05 / TMEM primitives shared by the tensor-core kernels of this library (rollout_tc2.cuh, dense_tc.cuh):
-// operand descriptors of the canonical plane layout, the MMA issue helpers, the fp32 -> three-plane split and the
-// transposing warp reduction.  (Round 1's cooperative 512-thread kernel that lived here is replaced by rollout_tc2.cuh.)
+// BF16x3 operand primitives of the warpgroup tensor-core kernels (rollout_tc2.cuh, dense_tc.cuh): operand descriptors
+// of the canonical plane layout, the fp32 -> three-plane split and the transposing warp reduction.
 //
 // Arithmetic: BF16x3.  x = b0 + b1 + b2 (three bf16 planes, residual <= 2^-27 |x|), a product keeps the six terms of
-// order <= 2 (b0b0, b0b1, b1b0, b1b1, b0b2, b2b0; neglected <= 2^-26), FP32 accumulation in TMEM: at least as accurate
-// as the 3xTF32 split of the other paths (parity tests hold it to the same bars).  Why bf16 and not tf32: tcgen05 reads
-// a 16-bit operand transposed (MN-major) from the plain no-swizzle layout, so ONE shared-memory buffer [sample][feature]
-// serves the layer products (K-major: contraction over features) and the weight-gradient products (MN-major:
-// contraction over samples); 32-bit operands need a second, 128B_BASE32B copy of every activation, which does not fit
-// (tools/umma_probe*.cu, profiles/r01_umma_probe*.txt).
+// order <= 2 (b0b0, b0b1, b1b0, b1b1, b0b2, b2b0; neglected <= 2^-26), FP32 accumulation: at least as accurate as the
+// 3xTF32 split of the other paths (parity tests hold it to the same bars).  Why bf16 and not tf32: wgmma reads a 16-bit
+// operand transposed (MN-major) from the plain no-swizzle layout, so ONE shared-memory buffer [sample][feature] serves
+// the layer products (K-major: contraction over features) and the weight-gradient products (MN-major: contraction over
+// samples); 32-bit operands are K-major only.
 //
 // Operand layout: plane[p][k/8][row][8] bf16 (p = 0..2), i.e. the no-swizzle canonical layout with chunk stride
 // rows*16 B and 8-row group stride 128 B.  K-major view: rows = M/N, K along k.  MN-major view (same bytes): M/N along
-// k, K = rows.  Thread (q, c) of the CTA owns sample r = 32 q + lane and the 16-column slice c: it writes two 16-byte
-// chunks per plane (a warp covers 512 contiguous bytes).
-//
-// Weight gradients: A = [delta_b0 | delta_b1] stacked to M = 128 (planes are contiguous), so one MMA does two terms;
-// rows 0..63 of the accumulator collect b0.(B0+B1+B2) + b2.B0 (the b2 MMA disables output lanes 64..127), rows 64..127
-// collect b1.(B0+B1+B2); the kernel epilogue adds the halves.  Bias gradients: B = `ones`.
+// k, K = rows (wgmma.cuh).
 #pragma once
 #include "rollout.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace gops {
 
 namespace tcf {
-constexpr uint32_t ACC = 0, D1S = 64, D2S = 128, H2S = 192, DW2 = 256, DB2 = 320, DW1 = 336, DB1 = 352, COLS = 512;
 constexpr int K1 = 16;                           // layer-1 K extent (inputs padded to 16)
 constexpr int HPLANE = 8 * 128 * 16;             // bytes of one hidden-activation plane ([8 chunks][128 rows][16 B])
 constexpr int XPLANE = 2 * 128 * 16;             // bytes of one observation plane
 constexpr int W2PLANE = 8 * 64 * 16, W1PLANE = 2 * 64 * 16;
-constexpr int RED = 4 * (MAXA * 64 + MAXA);      // floats: quarter partials of dW3 / db3
 constexpr int ONES_B = 2 * 16 * 16;              // bytes: [2 mn-groups][16 rows][16 B]
-}  // namespace tcf
-
-namespace tcf {
-
-__host__ __device__ constexpr uint32_t idesc_bf16(int M, int N, bool a_mn, bool b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// D[tmem] (+)= A . B^T, kind::f16 (bf16 operands, K = 16), `upper_off`: do not write accumulator lanes 64..127
-__device__ __forceinline__ void mma_bf16(uint32_t d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc,
-                                         bool upper_off = false) {
-  const uint32_t m = upper_off ? 0xffffffffu : 0u;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, {%5, %6, %7, %8}, p;\n\t}\n" ::"r"(d),
-      "l"(a), "l"(b), "r"(idesc), "r"(acc), "r"(0), "r"(0), "r"(m), "r"(m)
-      : "memory");
-}
 
 struct Op {            // one operand: smem address of plane 0, plane stride, descriptor strides, advance per K = 16 step
   uint32_t base, pstride, lbo, sbo, kadv;
@@ -67,45 +40,11 @@ __device__ __forceinline__ Op mn_w(const unsigned char* b, int plane_bytes) {   
   return Op{smem_u32(b), (uint32_t)plane_bytes, 128u, 1024u, 256u};
 }
 __device__ __forceinline__ uint64_t dsc(const Op& o, int plane) {
-  return umma::smem_desc(o.base + plane * o.pstride, o.lbo, o.sbo);
+  return wg::smem_desc(o.base + plane * o.pstride, o.lbo, o.sbo);
 }
 
-// D = A . B^T with the six BF16x3 terms (small ones first), KS steps of K = 16; the first MMA overwrites D
-template <int KS>
-__device__ __forceinline__ void issue6(uint32_t d, const Op& A, const Op& B, uint32_t idesc) {
-  const uint64_t a0 = dsc(A, 0), a1 = dsc(A, 1), a2 = dsc(A, 2), b0 = dsc(B, 0), b1 = dsc(B, 1), b2 = dsc(B, 2);
-  const uint64_t ka = A.kadv >> 4, kb = B.kadv >> 4;
-#pragma unroll
-  for (int ks = 0; ks < KS; ++ks) mma_bf16(d, a2 + ks * ka, b0 + ks * kb, idesc, ks > 0 ? 1u : 0u);
-#pragma unroll
-  for (int ks = 0; ks < KS; ++ks) mma_bf16(d, a0 + ks * ka, b2 + ks * kb, idesc, 1u);
-#pragma unroll
-  for (int ks = 0; ks < KS; ++ks) mma_bf16(d, a1 + ks * ka, b1 + ks * kb, idesc, 1u);
-#pragma unroll
-  for (int ks = 0; ks < KS; ++ks) mma_bf16(d, a1 + ks * ka, b0 + ks * kb, idesc, 1u);
-#pragma unroll
-  for (int ks = 0; ks < KS; ++ks) mma_bf16(d, a0 + ks * ka, b1 + ks * kb, idesc, 1u);
-#pragma unroll
-  for (int ks = 0; ks < KS; ++ks) mma_bf16(d, a0 + ks * ka, b0 + ks * kb, idesc, 1u);
-}
-// D = [A_b0 | A_b1]-stacked^T . (B0 + B1 + B2) + (A_b2^T . B0 on lanes 0..63), 8 steps of 16 samples
-// (`fresh`: the first MMA overwrites D -- the accumulators were just flushed, see tcf_flush)
-__device__ __forceinline__ void issue_stack(uint32_t d, const Op& A, const Op& B, uint32_t idesc, int bplanes,
-                                            uint32_t fresh) {
-  const uint64_t a01 = dsc(A, 0), a2 = dsc(A, 2), ka = A.kadv >> 4, kb = B.kadv >> 4;
-  for (int p = bplanes - 1; p >= 0; --p) {
-    const uint64_t b = dsc(B, p);
-#pragma unroll
-    for (int ks = 0; ks < 8; ++ks)
-      mma_bf16(d, a01 + ks * ka, b + ks * kb, idesc, (fresh && p == bplanes - 1 && ks == 0) ? 0u : 1u);
-  }
-  const uint64_t b0 = dsc(B, 0);
-#pragma unroll
-  for (int ks = 0; ks < 8; ++ks) mma_bf16(d, a2 + ks * ka, b0 + ks * kb, idesc, 1u, true);
-}
-
-// (x0, x1) -> packed bf16x2 words of the three planes (low half = x0); the residuals x - hi are formed by one packed
-// FMA per pair (hi * -1 + x: the same rounding as the subtraction)
+// (x0, x1) -> packed bf16x2 words of the three planes (low half = x0); the residuals x - hi are formed by one pair
+// FMA (hi * -1 + x: the same rounding as the subtraction)
 __device__ __forceinline__ f32x2::u64 bf16x2_as_f32x2(uint32_t p) {
   return f32x2::pk(__uint_as_float(p << 16), __uint_as_float(p & 0xffff0000u));
 }
@@ -123,6 +62,7 @@ __device__ __forceinline__ void split3(f32x2::u64 X, uint32_t& p0, uint32_t& p1,
 __device__ __forceinline__ void split3(float x0, float x1, uint32_t& p0, uint32_t& p1, uint32_t& p2) {
   split3(f32x2::pk(x0, x1), p0, p1, p2);
 }
+
 // 16 values of thread (q, c) -> its two 16-byte chunks (kc = 2c, 2c+1) of row r in the three planes of `buf`
 __device__ __forceinline__ void store16(unsigned char* buf, int plane_bytes, int c, int r, const float* v) {
   uint32_t w[3][8];

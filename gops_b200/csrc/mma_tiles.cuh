@@ -20,7 +20,7 @@ __device__ __forceinline__ void mma_tf32(float* d, const uint32_t* a, const uint
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 // x = hi + lo exactly; hi carries the top 11 mantissa bits (round-to-nearest, ties away: integer add of half an ulp,
-// then mask -- 2 instructions; cvt.rna.tf32.f32 compiles to 4 on sm_100a because it also screens Inf/NaN, which
+// then mask -- 2 instructions; cvt.rna.tf32.f32 takes more instructions because it also screens Inf/NaN, which
 // poison the result either way here), the tensor core truncates lo
 __device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
   hi = (__float_as_uint(x) + 0x1000u) & 0xffffe000u;

@@ -1,4 +1,4 @@
-// Fused rollout + loss + gradient kernel for hidden width 64 (sm_100a): shared-memory tile primitives.
+// Fused rollout + loss + gradient kernel for hidden width 64 (sm_90a): shared-memory tile primitives.
 //
 // One CTA owns chunks of NT samples (one per thread) for the whole horizon:
 //   * per-sample model state lives in the registers of its thread for all H steps;
@@ -81,7 +81,6 @@ struct KParams {
   int part_stride;
   // smem carve (floats)
   int w_floats, dw_floats, inp_max;
-  long long* dbg;          // development aid (GOPS_B200_TIMELINE): clock64 stamps of one owner and one helper thread
   // trace outputs (alg == ALG_TRACE)
   float* tr_obs; float* tr_act; float* tr_rew; float* tr_done;
   // constrained FHADP variants (fhadp_exterior / fhadp_lagrangian / fhadp_interior.py): 0 none, 1 exterior penalty,

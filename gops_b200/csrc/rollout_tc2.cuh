@@ -1,34 +1,28 @@
-// Pipelined tcgen05 / TMEM rollout kernel (64-wide nets, <= 16 inputs, state == obs models): TWO INDEPENDENT 256-thread
-// groups per CTA, each owning one 128-sample sub-tile at a time.
+// Fused wgmma rollout kernel (64-wide nets, <= 16 inputs, state == obs models): one 256-thread group per CTA owning one
+// 128-sample sub-tile at a time.
 //
-//   row = sample = TMEM lane.  Each sample row is served by a thread PAIR (h = 0 owner, h = 1 helper; both sit on the
-//   row's TMEM lane quarter).  The owner keeps the sample's model state and adjoint in registers for the whole
-//   horizon, runs the dynamics / adjoint and writes the observation row straight into the bf16x3 operand planes; owner
-//   and helper each read their 32 accumulator columns of the row back (tcgen05.ld 32x32b: lane = row), apply bias /
-//   activation / output layer and multiply their deltas.  No observation / action tiles in shared memory; the only
-//   exchange is the helper's half of the output dot product and the owner's output adjoint (2 KB per group).
-//   The reductions over samples run on the tensor core (dW1, db1, dW2, db2: contraction over the 128 samples with the
-//   MN-major view of the same operand planes) or as warp shuffles (dW3, db3).
+//   row = sample.  Each sample row is served by a thread PAIR (h = 0 owner in warpgroup 0, h = 1 helper in warpgroup 1,
+//   both with r = thread index in the warpgroup).  The owner keeps the sample's model state and adjoint in registers
+//   for the whole horizon, runs the dynamics / adjoint and writes the observation row straight into the bf16x3 operand
+//   planes; owner and helper each read their 32 accumulator columns of the row back, apply bias / activation / output
+//   layer and multiply their deltas.  The only other exchange is the helper's half of the output dot product and the
+//   owner's output adjoint (4 KB).
 //
-//   While one group waits for its MMA round trip (issue -> tensor pipe -> commit -> mbarrier), the other group's
-//   warps run their epilogue or dynamics: the two groups are never synchronised with each other (FHADP), so the tensor
-//   pipe and the CUDA cores overlap without any software pipelining.  Round 1's kernel marched all 512 threads through
-//   five issue -> wait -> epilogue round trips of ONE sub-tile (tensor pipe 17 % busy, issue slots 43 % busy).
-//   MMA issue is warp-uniform (group / warp ids come from __shfl_sync so that the descriptors live in uniform
-//   registers; one elected lane issues): the first version issued from `if (thread == 0)` and ptxas wrapped every
-//   UTCHMMA in a 9-instruction ELECT / R2UR.BROADCAST waterfall loop on the critical path.
+//   Every dense product is a warpgroup MMA (wgmma, M = 64): warpgroup h computes rows [64 h, 64 h + 64) of the 128-row
+//   layer / delta / input-gradient products and stores its register fragments into a row-major fp32 accumulator tile in
+//   shared memory, from which the row owners read.  The reductions over samples run on the tensor core as well
+//   (MN-major view of the same operand planes): warpgroup 0 forms dW2 / dW1, warpgroup 1 db2 / db1 (against a column
+//   of ones), and each adds its fragment straight into the group's FP32 global partial after every horizon step.
+//   dW3 / db3 are warp shuffles.
 //
-// Arithmetic (unchanged bars: loss 1e-4, gradient 2e-4 against the CPU oracle):
+// Arithmetic (bars: loss 1e-4, gradient 2e-4 against the CPU oracle):
 //   layer products        x . W^T      BF16x3 x BF16x3, six terms (FP32-accurate; the loss depends on these)
 //   delta / input grad    delta . W    delta in TWO bf16 planes (2^-17 relative: the gradient bar is 2e-4), W in three
-//   weight gradients      delta^T . h  [delta_b0 | delta_b1] stacked to M = 128 against (h_b0 + h_b1): four terms
-//   TMEM accumulators of the weight gradients are flushed into the group's FP32 global partial every FLUSH_EVERY
-//   horizon steps (the tensor core truncates when it adds into its accumulator, see DESIGN.md).
+//   weight gradients      delta^T . h  (delta_b0 + delta_b1) . (h_b0 + h_b1): four terms, FP32 accumulation
 //
-// Shared memory (C1: 221 KB of 227): weights 31.5 KB (TMA-staged, shared by both groups) + per group: H1 planes 48 KB,
-// delta planes 32 KB (delta2, then delta1 in the same buffer once the MMAs reading delta2 have retired), observation
-// planes 12 KB, exchange 2 KB.  TMEM: 240 of 256 columns per group (ACC 64 | act'(layer 1) 64 | dW2 64 | db2 16 |
-// dW1 16 | db1 16).
+// Shared memory (~206 KB of 227): weights 31.5 KB (TMA-staged) + H1 planes 48 KB, delta planes 32 KB (delta2, then delta1
+// in the same buffer), observation planes 12 KB, exchange 4 KB, accumulator tiles: products 34 KB, act'(layer 1) 34 KB,
+// input gradient 10 KB.
 #pragma once
 #include "models.cuh"
 #include "mlp_tc_full.cuh"
@@ -36,19 +30,16 @@
 namespace gops {
 namespace tc2 {
 
-constexpr int GT = 128;                 // rows (= samples) per sub-tile = UMMA M
-constexpr int GTH = 256;                // threads per group: owner half (h = 0) + helper half (h = 1)
-constexpr int NG = 2;                   // groups per CTA
+constexpr int GT = 128;                 // rows (= samples) per sub-tile = two wgmma M = 64 halves
+constexpr int GTH = 256;                // threads per group: owner warpgroup (h = 0) + helper warpgroup (h = 1)
+constexpr int NG = 1;                   // groups per CTA
 constexpr int NT2 = GTH * NG;
-constexpr uint32_t C_ACC = 0, C_D1 = 64, C_DW2 = 128, C_DB2 = 192, C_DW1 = 208, C_DB1 = 224, C_DX = 240, C_GROUP = 256;
+constexpr int AS = 68, XS = 20;         // row strides (floats) of the accumulator tiles (padded: conflict-free row reads)
 constexpr int HPL = tcf::HPLANE, XPL = tcf::XPLANE;
 constexpr int P_BYTES = 3 * HPL, Q_BYTES = 2 * HPL, XP_BYTES = 3 * XPL;
 constexpr int XCH_BYTES = 2 * GT * MAXA * 4;   // helper -> owner output partials | owner -> helper output adjoints
-constexpr int GROUP_BYTES = P_BYTES + Q_BYTES + XP_BYTES + XCH_BYTES;
-constexpr int FLUSH_EVERY = 30;         // horizon steps between flushes of the TMEM weight-gradient accumulators
-                                        // (<= 30 x 24 truncating accumulations per element.  Measured on the golden cases,
-                                        //  forced onto this kernel: gradient rel. L2 error 3.2e-6 at 15 steps, 4.8e-6 at 30,
-                                        //  bars 2e-4; every 8 steps cost 4 % more time; round 1's whole-kernel chain: 1.3e-4)
+constexpr int ACC_BYTES = GT * AS * 4, DX_BYTES = GT * XS * 4;
+constexpr int GROUP_BYTES = P_BYTES + Q_BYTES + XP_BYTES + XCH_BYTES + 2 * ACC_BYTES + DX_BYTES;
 constexpr int HDR_BYTES = 256;
 
 __host__ __device__ inline size_t smem_bytes(int w_floats) {
@@ -56,36 +47,6 @@ __host__ __device__ inline size_t smem_bytes(int w_floats) {
 }
 
 __device__ __forceinline__ void group_sync(int g) { asm volatile("bar.sync %0, 256;" ::"r"(1 + g) : "memory"); }
-// Issue order of the two MMA streams of a backward stage: warp 0 (critical-path product) arrives after its commit,
-// warp 1 (weight-gradient products, twice the work) issues behind it -- the tensor pipe executes in arrival order, and
-// a critical product queued behind the weight gradients costs the whole group ~1 k cycles per stage.
-__device__ __forceinline__ void order_arrive(int g) { asm volatile("bar.arrive %0, 64;" ::"r"(3 + g) : "memory"); }
-__device__ __forceinline__ void order_wait(int g) { asm volatile("bar.sync %0, 64;" ::"r"(3 + g) : "memory"); }
-using umma::elect_one;
-
-// 16 accumulator columns of this thread's lane, WITHOUT waiting (issue several, then tm_wait_ld once)
-__device__ __forceinline__ void tm_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "[%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tm_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// 32 columns -> floats (two x16 loads in flight, one wait)
-__device__ __forceinline__ void tm_ld32(uint32_t taddr, float* v) {
-  uint32_t r[32];
-  tm_ld16(taddr, r);
-  tm_ld16(taddr + 16, r + 16);
-  tm_wait_ld();
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tm_st32(uint32_t taddr, const float* v) {
-  umma::tmem_st16(taddr, v);
-  umma::tmem_st16(taddr + 16, v + 16);
-}
 
 // (x0, x1) -> packed bf16x2 words of two planes (low half = x0)
 __device__ __forceinline__ void split2(f32x2::u64 X, uint32_t& p0, uint32_t& p1) {
@@ -95,83 +56,114 @@ __device__ __forceinline__ void split2(f32x2::u64 X, uint32_t& p0, uint32_t& p1)
   f32x2::upk(f32x2::fma(tcf::bf16x2_as_f32x2(p0), f32x2::rep(-1.f), X), r0, r1);
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(p1) : "f"(r1), "f"(r0));
 }
-__device__ __forceinline__ void split2(float x0, float x1, uint32_t& p0, uint32_t& p1) { split2(f32x2::pk(x0, x1), p0, p1); }
 
 // Per-thread view of its group's resources.  g, h, wg are warp-uniform (derived from a __shfl_sync'ed warp id).
 struct Grp {
   unsigned char *P, *Q, *Xp;        // H1 planes (3), delta planes (2), observation planes (3)
   float *zp, *zb;                   // exchange: helper -> owner output partials [128][MAXA]; owner -> helper adjoints
+  float *A, *D1, *DX;               // accumulator tiles: products [128][AS], act'(layer 1) [128][AS], input gradient [128][XS]
   const unsigned char* ones;
-  uint64_t *bc, *bd2, *bd1, *bdx;   // mbarriers: critical-path MMA groups / dW2+db2 / dW1+db1 / deferred input gradient
-  uint32_t pc, pd2, pd1, pdx;       // their phases
-  uint32_t tm;                      // TMEM address of this thread's lane, column 0 of the group
-  uint32_t tmg;                     // TMEM address lane 0, column 0 of the group (MMA destinations)
-  uint32_t fresh;                   // 1: the next weight-gradient MMAs overwrite their accumulators
-  bool d2_pending, d1_pending;      // weight-gradient MMA groups in flight (their operand planes must not be rewritten)
   int g, h, wg, r;                  // group, half (0 owner / 1 helper), warp in group, row (= sample of the sub-tile)
-#ifdef GOPS_TC2_TIMELINE
-  long long* dbg;                   // timeline stamps (development aid)
-  int dbgn;
-#endif
   // staged weights of the network in use
   const unsigned char *W1, *W2;
   const float *W3, *b1, *b2, *b3;
 };
 
-// timeline stamp: (clock << 8) | id, only for the two instrumented threads and only when a buffer was attached
-// (compiled in with -DGOPS_TC2_TIMELINE only: tools/timeline_report.py; profiles/r02_tc2_timeline.txt)
-__device__ __forceinline__ void TL(Grp& G, int id) {
-#ifdef GOPS_TC2_TIMELINE
-  if (G.dbg != nullptr && G.dbgn < 4000) G.dbg[G.dbgn++] = (clock64() << 8) | (long long)id;
-#else
-  (void)G; (void)id;
-#endif
-}
 __device__ __forceinline__ void bind(Grp& G, const float* Wsm, const NetL& L) {
   G.W1 = reinterpret_cast<const unsigned char*>(Wsm + L.o_w1);
   G.W2 = reinterpret_cast<const unsigned char*>(Wsm + L.o_w2);
   G.W3 = Wsm + L.o_w3; G.b1 = Wsm + L.o_b1; G.b2 = Wsm + L.o_b2; G.b3 = Wsm + L.o_b3;
 }
-__device__ __forceinline__ void wait_c(Grp& G) { mbar_wait(G.bc, G.pc); G.pc ^= 1u; umma::fence_after_sync(); }
-__device__ __forceinline__ void wait_d2(Grp& G) {
-  if (G.d2_pending) { mbar_wait(G.bd2, G.pd2); G.pd2 ^= 1u; umma::fence_after_sync(); G.d2_pending = false; }
-}
-__device__ __forceinline__ void wait_d1(Grp& G) {
-  if (G.d1_pending) { mbar_wait(G.bd1, G.pd1); G.pd1 ^= 1u; umma::fence_after_sync(); G.d1_pending = false; }
-}
-// make this thread's shared-memory / TMEM writes visible to the MMA issuer, then meet the group
+// make this thread's shared-memory writes visible to the tensor core, then meet the group
 __device__ __forceinline__ void publish(const Grp& G) {
   fence_proxy_async();
-  umma::fence_before_sync();
   group_sync(G.g);
 }
 
-// delta (2 planes, K-major A) x W^T (MN-major B): a1b0, a0b1, a0b0 -- small terms first.  The dropped terms (a1b1, a0b2)
-// are 2^-17 relative, the size of delta's own two-plane truncation; these products sit on the serial chain of the
-// reverse sweep (delta2 -> delta1 -> dX -> lambda), so 12 MMAs instead of 20 shorten every reverse step.
-template <int KS>
-__device__ __forceinline__ void issue_dw(uint32_t d, const tcf::Op& A, const tcf::Op& B, uint32_t idesc) {
+// A . B^T with the six BF16x3 terms (small ones first), KS steps of K = 16; A K-major (this warpgroup's 64 rows)
+template <int N, int TB, int KS>
+__device__ __forceinline__ void mma6(float* d, const tcf::Op& A, const tcf::Op& B) {
+  using namespace tcf;
+  const uint64_t a0 = dsc(A, 0), a1 = dsc(A, 1), a2 = dsc(A, 2), b0 = dsc(B, 0), b1 = dsc(B, 1), b2 = dsc(B, 2);
+  const uint64_t ka = A.kadv >> 4, kb = B.kadv >> 4;
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) wg::mma_bf16<N, 0, TB>(d, a2 + ks * ka, b0 + ks * kb, ks > 0 ? 1u : 0u);
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) wg::mma_bf16<N, 0, TB>(d, a0 + ks * ka, b2 + ks * kb, 1u);
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) wg::mma_bf16<N, 0, TB>(d, a1 + ks * ka, b1 + ks * kb, 1u);
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) wg::mma_bf16<N, 0, TB>(d, a1 + ks * ka, b0 + ks * kb, 1u);
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) wg::mma_bf16<N, 0, TB>(d, a0 + ks * ka, b1 + ks * kb, 1u);
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) wg::mma_bf16<N, 0, TB>(d, a0 + ks * ka, b0 + ks * kb, 1u);
+}
+// delta (2 planes, K-major A) x W (MN-major B): a1b0, a0b1, a0b0 -- small terms first.  The dropped terms (a1b1, a0b2)
+// are 2^-17 relative, the size of delta's own two-plane truncation.
+template <int N, int KS>
+__device__ __forceinline__ void mma_dw(float* d, const tcf::Op& A, const tcf::Op& B) {
   using namespace tcf;
   const uint64_t a0 = dsc(A, 0), a1 = dsc(A, 1), b0 = dsc(B, 0), b1 = dsc(B, 1);
   const uint64_t ka = A.kadv >> 4, kb = B.kadv >> 4;
 #pragma unroll
-  for (int ks = 0; ks < KS; ++ks) mma_bf16(d, a1 + ks * ka, b0 + ks * kb, idesc, ks > 0 ? 1u : 0u);
+  for (int ks = 0; ks < KS; ++ks) wg::mma_bf16<N, 0, 1>(d, a1 + ks * ka, b0 + ks * kb, ks > 0 ? 1u : 0u);
 #pragma unroll
-  for (int ks = 0; ks < KS; ++ks) mma_bf16(d, a0 + ks * ka, b1 + ks * kb, idesc, 1u);
+  for (int ks = 0; ks < KS; ++ks) wg::mma_bf16<N, 0, 1>(d, a0 + ks * ka, b1 + ks * kb, 1u);
 #pragma unroll
-  for (int ks = 0; ks < KS; ++ks) mma_bf16(d, a0 + ks * ka, b0 + ks * kb, idesc, 1u);
+  for (int ks = 0; ks < KS; ++ks) wg::mma_bf16<N, 0, 1>(d, a0 + ks * ka, b0 + ks * kb, 1u);
 }
-// D (+)= [A_b0 | A_b1]^T (M = 128 stacked, MN-major) . (B_b0 + .. + B_b{BP-1}), 8 steps of 16 samples
-template <int BP>
-__device__ __forceinline__ void issue_wgrad(uint32_t d, const tcf::Op& A, const tcf::Op& B, uint32_t idesc, uint32_t fresh) {
+// weight gradient over the sub-tile's 128 samples: D = (A_b0 + A_b1)^T . (B_b0 + .. + B_b{BP-1}), both MN-major
+template <int N, int BP>
+__device__ __forceinline__ void mma_wgrad(float* d, const tcf::Op& A, const tcf::Op& B) {
   using namespace tcf;
-  const uint64_t a01 = dsc(A, 0), ka = A.kadv >> 4, kb = B.kadv >> 4;
+  const uint64_t ka = A.kadv >> 4, kb = B.kadv >> 4;
+  uint32_t acc = 0u;
 #pragma unroll
-  for (int p = BP - 1; p >= 0; --p) {
-    const uint64_t b = dsc(B, p);
+  for (int p = BP - 1; p >= 0; --p)
 #pragma unroll
-    for (int ks = 0; ks < 8; ++ks)
-      mma_bf16(d, a01 + ks * ka, b + ks * kb, idesc, (p == BP - 1 && ks == 0) ? (fresh ? 0u : 1u) : 1u);
+    for (int q = 1; q >= 0; --q) {
+      const uint64_t a = dsc(A, q), b = dsc(B, p);
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks) { wg::mma_bf16<N, 1, 1>(d, a + ks * ka, b + ks * kb, acc); acc = 1u; }
+    }
+}
+// this warpgroup's fragment of a 128-row product -> rows [64 h, 64 h + 64) of a row-major tile
+template <int N>
+__device__ __forceinline__ void store_frag(const Grp& G, float* dst, int ld, const float* d) {
+#pragma unroll
+  for (int i = 0; i < N / 2; i += 2)
+    *reinterpret_cast<float2*>(dst + (64 * G.h + wg::frag_row(G.r, i)) * ld + wg::frag_col(G.r, i)) = make_float2(d[i], d[i + 1]);
+}
+// this warpgroup's fragment of a [64 output rows][N] weight gradient added into the FP32 partial (row stride ld,
+// columns < ncols)
+template <int N>
+__device__ __forceinline__ void add_frag(float* __restrict__ dst, int ld, int ncols, const float* d, int r) {
+#pragma unroll
+  for (int i = 0; i < N / 2; ++i) {
+    const int row = wg::frag_row(r, i), col = wg::frag_col(r, i);
+    if (col < ncols) dst[row * ld + col] += d[i];
+  }
+}
+// the group's 128-row product A . B^T (A = k_act(...) planes, six terms) into the product tile; ends with the group
+// barrier: the results are visible and every wgmma operand read has retired
+template <int KS>
+__device__ __forceinline__ void layer_product(const Grp& G, const tcf::Op& Ain, const tcf::Op& B) {
+  tcf::Op A = Ain;
+  A.base += 1024u * G.h;                          // + 8 row groups of 128 B
+  float d[32];
+  wg::fence();
+  mma6<64, 0, KS>(d, A, B);
+  wg::commit();
+  wg::wait<0>();
+  store_frag<64>(G, G.A, AS, d);
+  group_sync(G.g);
+}
+__device__ __forceinline__ void read16(const float* src, float* v) {
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const float4 x = reinterpret_cast<const float4*>(src)[q];
+    v[4 * q] = x.x; v[4 * q + 1] = x.y; v[4 * q + 2] = x.z; v[4 * q + 3] = x.w;
   }
 }
 
@@ -191,13 +183,10 @@ __device__ __forceinline__ void write_x_row(const Grp& G, const float* x, int nc
   }
 }
 
-// layer 1, first half: observation planes . W1^T issued; the caller may overlap work with the MMA before layer1_finish
+// layer 1, first half: observation planes . W1^T into the product tile
 template <int NS>
 __device__ __forceinline__ void layer1_issue(Grp& G, const NetL& L, const float* st, float vt) {
   using namespace tcf;
-  TL(G, 1);
-  wait_d1(G);                                   // the dW1 MMAs of the previous step still read the X planes
-  TL(G, 2);
   if (G.h == 0) {
     float x[16];
 #pragma unroll
@@ -209,41 +198,25 @@ __device__ __forceinline__ void layer1_issue(Grp& G, const NetL& L, const float*
     }
     write_x_row(G, x, L.in <= 8 ? 1 : 2);
   }
-  TL(G, 3);
   publish(G);
-  TL(G, 4);
-  if (G.wg == 0) {
-    if (elect_one()) {
-      umma::fence_after_sync();
-      issue6<1>(G.tmg + C_ACC, k_act(G.Xp, XPL), k_w(G.W1, W1PLANE), idesc_bf16(128, 64, false, false));
-      umma::commit(G.bc);
-    }
-  }
-  TL(G, 5);
+  layer_product<1>(G, k_act(G.Xp, XPL), k_w(G.W1, W1PLANE));
 }
-// AF: hidden activation fixed at compile time (>= 0), or -1 = dispatch on the runtime id.  The register allocation of the
-// kernel is decided by its most demanding path: with the activation fixed (the headline configurations use GELU) the other
-// six epilogue variants are not compiled in.
+// AF: hidden activation fixed at compile time (>= 0), or -1 = dispatch on the runtime id.  With the activation fixed (the
+// headline configurations use GELU) the other six epilogue variants are not compiled in.
 #define GOPS_TC2_ACT_SWITCH(AF, act, M)     \
   if constexpr ((AF) >= 0) { M(AF); }       \
   else { GOPS_ACT_SWITCH(act, M) }
 
-// layer 1, second half: + b1, activation -> this thread's 32 columns of the H1 planes (FULL: act' parked in TMEM).
-// Two rolled passes of 16 columns: half the code and half the registers of one 32-column pass (the kernel is
-// instruction-fetch sensitive: 8 warps per SM sub-partition pair run different phases of a long straight-line body).
+// layer 1, second half: + b1, activation -> this thread's columns of the H1 planes (FULL: act' into the D1 tile).
 // [lo, hi): the 16-column blocks of the row this thread converts (forward sweep: owner 0-1, helper 2-3; reverse sweep:
 // the helper takes all four while the owner runs the adjoint of the dynamics).
 template <bool FULL, int AF>
 __device__ __forceinline__ void layer1_finish(Grp& G, const NetL& L, int lo, int hi) {
   using namespace tcf;
-  TL(G, 6);
-  wait_d2(G);                                   // the dW2 MMAs of the previous step still read the H1 planes
-  wait_c(G);
-  TL(G, 7);
 #pragma unroll 1
   for (int c16 = lo; c16 < hi; ++c16) {
     float v[16], d[16];
-    umma::tmem_ld16(G.tm + C_ACC + 16 * c16, v);
+    read16(G.A + G.r * AS + 16 * c16, v);
     const float* bias = G.b1 + 16 * c16;
 #define GOPS_TC2_A1(A)                                                      \
   _Pragma("unroll") for (int e = 0; e < 16; e += 2) {                                         \
@@ -254,10 +227,12 @@ __device__ __forceinline__ void layer1_finish(Grp& G, const NetL& L, int lo, int
     GOPS_TC2_ACT_SWITCH(AF, L.hact, GOPS_TC2_A1)
 #undef GOPS_TC2_A1
     store16(G.P, HPL, c16, G.r, v);
-    if constexpr (FULL) umma::tmem_st16(G.tm + C_D1 + 16 * c16, d);
+    if constexpr (FULL) {
+#pragma unroll
+      for (int q = 0; q < 4; ++q)
+        reinterpret_cast<float4*>(G.D1 + G.r * AS + 16 * c16)[q] = make_float4(d[4 * q], d[4 * q + 1], d[4 * q + 2], d[4 * q + 3]);
+    }
   }
-  if constexpr (FULL) umma::tmem_wait_st();
-  TL(G, 8);
 }
 
 // layer 2 + output layer, forward only: the owner gets z[a] = b3[a] + W3[a] . act(H1 . W2^T + b2)
@@ -265,16 +240,7 @@ template <int AF>
 __device__ __forceinline__ void layer2_out(Grp& G, const NetL& L, float* z) {
   using namespace tcf;
   publish(G);
-  TL(G, 9);
-  if (G.wg == 0) {
-    if (elect_one()) {
-      umma::fence_after_sync();
-      issue6<4>(G.tmg + C_ACC, k_act(G.P, HPL), k_w(G.W2, W2PLANE), idesc_bf16(128, 64, false, false));
-      umma::commit(G.bc);
-    }
-  }
-  wait_c(G);
-  TL(G, 10);
+  layer_product<4>(G, k_act(G.P, HPL), k_w(G.W2, W2PLANE));
   float zp[MAXA];
 #pragma unroll
   for (int a = 0; a < MAXA; ++a) zp[a] = 0.f;
@@ -282,7 +248,7 @@ __device__ __forceinline__ void layer2_out(Grp& G, const NetL& L, float* z) {
   for (int cb = 0; cb < 2; ++cb) {
     const int c16 = 2 * G.h + cb;
     float v[16];
-    umma::tmem_ld16(G.tm + C_ACC + 16 * c16, v);
+    read16(G.A + G.r * AS + 16 * c16, v);
     const float* bias = G.b2 + 16 * c16;
 #define GOPS_TC2_A2(A)                               \
   _Pragma("unroll") for (int e = 0; e < 16; e += 2)  \
@@ -306,10 +272,7 @@ __device__ __forceinline__ void layer2_out(Grp& G, const NetL& L, float* z) {
     for (int a = 0; a < MAXA; ++a)
       if (a < L.out) G.zp[G.r * MAXA + a] = zp[a];
   }
-  umma::fence_before_sync();      // the accumulator reads are ordered before the next MMA group (issued after a barrier)
-  TL(G, 11);
   group_sync(G.g);
-  TL(G, 12);
   if (G.h == 0) {
 #pragma unroll
     for (int a = 0; a < MAXA; ++a) z[a] = a < L.out ? G.b3[a] + (zp[a] + G.zp[G.r * MAXA + a]) : 0.f;
@@ -334,22 +297,12 @@ __device__ __forceinline__ void layer2_back(Grp& G, const NetL& L, const float* 
     for (int a = 0; a < MAXA; ++a)
       if (a < L.out) G.zb[G.r * MAXA + a] = zbar[a];
   }
-  TL(G, 13);
   publish(G);
-  TL(G, 14);
-  if (G.wg == 0) {
-    if (elect_one()) {
-      umma::fence_after_sync();
-      issue6<4>(G.tmg + C_ACC, k_act(G.P, HPL), k_w(G.W2, W2PLANE), idesc_bf16(128, 64, false, false));
-      umma::commit(G.bc);
-    }
-  }
+  layer_product<4>(G, k_act(G.P, HPL), k_w(G.W2, W2PLANE));
   float zb[MAXA];
 #pragma unroll
   for (int a = 0; a < MAXA; ++a) zb[a] = a < L.out ? G.zb[G.r * MAXA + a] : 0.f;
   const int lane = G.r & 31;
-  wait_c(G);
-  TL(G, 15);
   float zp[MAXA];
 #pragma unroll
   for (int a = 0; a < MAXA; ++a) zp[a] = 0.f;
@@ -357,7 +310,7 @@ __device__ __forceinline__ void layer2_back(Grp& G, const NetL& L, const float* 
   for (int cb = 0; cb < 2; ++cb) {
     const int c16 = 2 * G.h + cb;
     float v[16], d[16];
-    umma::tmem_ld16(G.tm + C_ACC + 16 * c16, v);
+    read16(G.A + G.r * AS + 16 * c16, v);
     const float* bias = G.b2 + 16 * c16;
 #define GOPS_TC2_A3(A)                               \
   _Pragma("unroll") for (int e = 0; e < 16; e += 2)  \
@@ -434,205 +387,119 @@ __device__ __forceinline__ void layer2_back(Grp& G, const NetL& L, const float* 
   }
 }
 
-// delta2 planes -> delta1 = (delta2 . W2) * act'(pre1) (same planes, once the readers of delta2 retired) ->
-// input gradient dx[0 .. 15] for the owner (want_dx) and the weight-gradient MMAs of both layers (WANT_DW).
-// defer_dx: the input-gradient product goes to its own TMEM columns (C_DX) and mbarrier and is NOT waited for here; the
-// owner picks it up with collect_dx() when it needs the adjoint (reverse sweep: after the next step's layer-1 MMAs were
-// issued), which takes one MMA round trip off the serial chain of every step.
+// delta2 planes -> delta1 = (delta2 . W2) * act'(pre1) (same planes, once the readers of delta2 retired) -> input
+// gradient rows in the DX tile (want_dx; the owner reads them with collect_dx) and, WANT_DW, the weight gradients of both
+// layers added into the group's partial `part`: warpgroup 0 forms dW2 / dW1, warpgroup 1 db2 / db1.
 template <bool WANT_DW>
-__device__ __forceinline__ void backprop(Grp& G, const NetL& L, bool want_dx, float* dx, bool defer_dx = false) {
+__device__ __forceinline__ void backprop(Grp& G, const NetL& L, bool want_dx, float* __restrict__ part) {
   using namespace tcf;
-  TL(G, 16);
   publish(G);
-  TL(G, 17);
-  if (G.wg == 0) {
-    if (elect_one()) {
-      umma::fence_after_sync();
-      issue_dw<4>(G.tmg + C_ACC, k_act(G.Q, HPL), mn_w(G.W2, W2PLANE), idesc_bf16(128, 64, false, true));
-      umma::commit(G.bc);
-    }
-    if constexpr (WANT_DW) order_arrive(G.g);
-  }
-  if constexpr (WANT_DW) {
-    if (G.wg == 1) {
-      order_wait(G.g);
-      if (elect_one()) {
-        umma::fence_after_sync();
-        const Op A = mn_act(G.Q, HPL);
-        issue_wgrad<2>(G.tmg + C_DW2, A, mn_act(G.P, HPL), idesc_bf16(128, 64, true, true), G.fresh);
-        const Op one{smem_u32(G.ones), 0u, 128u, 256u, 0u};
-        issue_wgrad<1>(G.tmg + C_DB2, A, one, idesc_bf16(128, 16, true, true), G.fresh);
-        umma::commit(G.bd2);
+  {
+    Op A = k_act(G.Q, HPL);
+    A.base += 1024u * G.h;
+    float d[32];
+    wg::fence();
+    mma_dw<64, 4>(d, A, mn_w(G.W2, W2PLANE));
+    wg::commit();
+    if constexpr (WANT_DW) {
+      const Op Ad = mn_act(G.Q, HPL);
+      if (G.h == 0) {
+        float w[32];
+        wg::fence();
+        mma_wgrad<64, 2>(w, Ad, mn_act(G.P, HPL));
+        wg::commit();
+        wg::wait<0>();
+        wg::reg_fence<32>(w);
+        add_frag<64>(part + L.g_w2, 64, 64, w, G.r);
+      } else {
+        float w[8];
+        wg::fence();
+        mma_wgrad<16, 1>(w, Ad, Op{smem_u32(G.ones), 0u, 128u, 256u, 0u});
+        wg::commit();
+        wg::wait<0>();
+        wg::reg_fence<8>(w);
+        add_frag<16>(part + L.g_b2, 1, 1, w, G.r);
       }
     }
-    G.d2_pending = true;
+    wg::wait<0>();
+    wg::reg_fence<32>(d);
+    store_frag<64>(G, G.A, AS, d);
   }
-  wait_c(G);
-  TL(G, 18);
-  uint32_t w0[16], w1[16];                       // delta1 planes of this thread's 32 columns, held until delta2's readers retired
+  group_sync(G.g);                               // delta2 . W2 visible; every reader of delta2 / H1 has retired
+  if (!WANT_DW && !want_dx) return;
   {
-    uint32_t ra[32], rb[32];
-    tm_ld16(G.tm + C_ACC + 32 * G.h, ra);
-    tm_ld16(G.tm + C_ACC + 32 * G.h + 16, ra + 16);
-    tm_ld16(G.tm + C_D1 + 32 * G.h, rb);
-    tm_ld16(G.tm + C_D1 + 32 * G.h + 16, rb + 16);
-    tm_wait_ld();
+    float ra[32], rb[32];
+    read16(G.A + G.r * AS + 32 * G.h, ra);
+    read16(G.A + G.r * AS + 32 * G.h + 16, ra + 16);
+    read16(G.D1 + G.r * AS + 32 * G.h, rb);
+    read16(G.D1 + G.r * AS + 32 * G.h + 16, rb + 16);
+    uint32_t w0[16], w1[16];                     // delta1 planes of this thread's 32 columns
 #pragma unroll
     for (int i = 0; i < 16; ++i)
-      split2(f32x2::mul(f32x2::pk(__uint_as_float(ra[2 * i]), __uint_as_float(ra[2 * i + 1])),
-                        f32x2::pk(__uint_as_float(rb[2 * i]), __uint_as_float(rb[2 * i + 1]))), w0[i], w1[i]);
-  }
-  if (!WANT_DW && !want_dx) {
-    umma::fence_before_sync();
-    return;
-  }
-  TL(G, 19);
-  wait_d2(G);                                    // dW2 / db2 have consumed delta2 (and the H1 planes)
-  TL(G, 20);
+      split2(f32x2::mul(f32x2::pk(ra[2 * i], ra[2 * i + 1]), f32x2::pk(rb[2 * i], rb[2 * i + 1])), w0[i], w1[i]);
 #pragma unroll
-  for (int c = 0; c < 4; ++c) {
-    *reinterpret_cast<uint4*>(G.Q + ((4 * G.h + c) * 128 + G.r) * 16) = make_uint4(w0[4 * c], w0[4 * c + 1], w0[4 * c + 2], w0[4 * c + 3]);
-    *reinterpret_cast<uint4*>(G.Q + HPL + ((4 * G.h + c) * 128 + G.r) * 16) = make_uint4(w1[4 * c], w1[4 * c + 1], w1[4 * c + 2], w1[4 * c + 3]);
+    for (int c = 0; c < 4; ++c) {
+      *reinterpret_cast<uint4*>(G.Q + ((4 * G.h + c) * 128 + G.r) * 16) = make_uint4(w0[4 * c], w0[4 * c + 1], w0[4 * c + 2], w0[4 * c + 3]);
+      *reinterpret_cast<uint4*>(G.Q + HPL + ((4 * G.h + c) * 128 + G.r) * 16) = make_uint4(w1[4 * c], w1[4 * c + 1], w1[4 * c + 2], w1[4 * c + 3]);
+    }
   }
   publish(G);
-  TL(G, 21);
-  if (G.wg == 0) {
-    if (want_dx) {
-      if (elect_one()) {
-        umma::fence_after_sync();
-        issue_dw<4>(G.tmg + (defer_dx ? C_DX : C_ACC), k_act(G.Q, HPL), mn_w(G.W1, W1PLANE), idesc_bf16(128, 16, false, true));
-        umma::commit(defer_dx ? G.bdx : G.bc);
-      }
-    }
-    if constexpr (WANT_DW) order_arrive(G.g);
+  if (want_dx) {
+    Op A = k_act(G.Q, HPL);
+    A.base += 1024u * G.h;
+    float d[8];
+    wg::fence();
+    mma_dw<16, 4>(d, A, mn_w(G.W1, W1PLANE));
+    wg::commit();
+    wg::wait<0>();
+    wg::reg_fence<8>(d);
+    store_frag<16>(G, G.DX, XS, d);
   }
   if constexpr (WANT_DW) {
-    if (G.wg == 1) {
-      order_wait(G.g);
-      if (elect_one()) {
-        umma::fence_after_sync();
-        const Op A = mn_act(G.Q, HPL);
-        issue_wgrad<2>(G.tmg + C_DW1, A, mn_act(G.Xp, XPL), idesc_bf16(128, 16, true, true), G.fresh);
-        const Op one{smem_u32(G.ones), 0u, 128u, 256u, 0u};
-        issue_wgrad<1>(G.tmg + C_DB1, A, one, idesc_bf16(128, 16, true, true), G.fresh);
-        umma::commit(G.bd1);
-      }
-    }
-    G.d1_pending = true;
-    G.fresh = 0u;
+    const Op Ad = mn_act(G.Q, HPL);
+    float w[8];
+    wg::fence();
+    if (G.h == 0) mma_wgrad<16, 2>(w, Ad, mn_act(G.Xp, XPL));
+    else mma_wgrad<16, 1>(w, Ad, Op{smem_u32(G.ones), 0u, 128u, 256u, 0u});
+    wg::commit();
+    wg::wait<0>();
+    wg::reg_fence<8>(w);
+    if (G.h == 0) add_frag<16>(part + L.g_w1, L.in, L.in, w, G.r);
+    else add_frag<16>(part + L.g_b1, 1, 1, w, G.r);
   }
-  if (want_dx && !defer_dx) {
-    wait_c(G);
-    TL(G, 22);
-    if (G.h == 0) {
-      uint32_t rr[16];
-      tm_ld16(G.tm + C_ACC, rr);
-      tm_wait_ld();
-#pragma unroll
-      for (int f = 0; f < 16; ++f) dx[f] = __uint_as_float(rr[f]);
-    }
-    umma::fence_before_sync();
-  }
+  group_sync(G.g);                               // input gradient visible; delta1 / X planes free
 }
 
-// owner half: the deferred input gradient of the previous backprop(..., defer_dx = true)
-__device__ __forceinline__ void collect_dx(Grp& G, float* dx) {
-  mbar_wait(G.bdx, G.pdx);
-  G.pdx ^= 1u;
-  umma::fence_after_sync();
-  uint32_t rr[16];
-  tm_ld16(G.tm + C_DX, rr);
-  tm_wait_ld();
+// owner half: the input gradient of the last backprop(..., want_dx = true)
+__device__ __forceinline__ void collect_dx(const Grp& G, float* dx) {
+  float v[16];
+  read16(G.DX + G.r * XS, v);
 #pragma unroll
-  for (int f = 0; f < 16; ++f) dx[f] = __uint_as_float(rr[f]);
-  umma::fence_before_sync();
-}
-
-// TMEM weight-gradient accumulators -> the group's FP32 global partial (torch flat layout), then mark them fresh.
-// Lanes 0..63 hold the delta_b0 share of gradient row j = lane, lanes 64..127 the delta_b1 share of row lane - 64;
-// thread (h, r) moves columns [32 h, 32 h + 32) of dW2, the owner half also dW1 / db2 / db1.
-__device__ __forceinline__ void flush(Grp& G, const NetL& L, float* __restrict__ part) {
-  TL(G, 23);
-  wait_d2(G);
-  wait_d1(G);
-  TL(G, 24);
-  if (G.fresh) return;                           // nothing accumulated since the last flush (uniform over the group)
-  float* S = reinterpret_cast<float*>(G.P);      // scratch [64][84]: the H1 planes are dead here
-  float w2[32], w1[16], bb[2];
-  {
-    uint32_t ra[32], rb[16], rc[16], rd[16];
-    tm_ld16(G.tm + C_DW2 + 32 * G.h, ra);
-    tm_ld16(G.tm + C_DW2 + 32 * G.h + 16, ra + 16);
-    if (G.h == 0) { tm_ld16(G.tm + C_DW1, rb); tm_ld16(G.tm + C_DB2, rc); tm_ld16(G.tm + C_DB1, rd); }
-    tm_wait_ld();
-#pragma unroll
-    for (int e = 0; e < 32; ++e) w2[e] = __uint_as_float(ra[e]);
-#pragma unroll
-    for (int e = 0; e < 16; ++e) w1[e] = G.h == 0 ? __uint_as_float(rb[e]) : 0.f;
-    bb[0] = G.h == 0 ? __uint_as_float(rc[0]) : 0.f;
-    bb[1] = G.h == 0 ? __uint_as_float(rd[0]) : 0.f;
-  }
-  umma::fence_before_sync();
-  if (G.r >= 64) {
-    float* row = S + (G.r - 64) * 84;
-#pragma unroll
-    for (int e4 = 0; e4 < 8; ++e4)
-      *reinterpret_cast<float4*>(row + 32 * G.h + 4 * e4) = make_float4(w2[4 * e4], w2[4 * e4 + 1], w2[4 * e4 + 2], w2[4 * e4 + 3]);
-    if (G.h == 0) {
-#pragma unroll
-      for (int e4 = 0; e4 < 4; ++e4)
-        *reinterpret_cast<float4*>(row + 64 + 4 * e4) = make_float4(w1[4 * e4], w1[4 * e4 + 1], w1[4 * e4 + 2], w1[4 * e4 + 3]);
-      row[80] = bb[0]; row[81] = bb[1];
-    }
-  }
-  group_sync(G.g);
-  if (G.r < 64) {
-    const float* row = S + G.r * 84;
-    float* pw2 = part + L.g_w2 + G.r * 64 + 32 * G.h;
-#pragma unroll
-    for (int e4 = 0; e4 < 8; ++e4) {
-      const float4 o = *reinterpret_cast<const float4*>(row + 32 * G.h + 4 * e4);
-      float4 c = *reinterpret_cast<float4*>(pw2 + 4 * e4);
-      c.x += w2[4 * e4] + o.x; c.y += w2[4 * e4 + 1] + o.y; c.z += w2[4 * e4 + 2] + o.z; c.w += w2[4 * e4 + 3] + o.w;
-      *reinterpret_cast<float4*>(pw2 + 4 * e4) = c;
-    }
-    if (G.h == 0) {
-      float* pw1 = part + L.g_w1 + G.r * L.in;
-#pragma unroll
-      for (int k = 0; k < 16; ++k)
-        if (k < L.in) pw1[k] += w1[k] + row[64 + k];
-      part[L.g_b2 + G.r] += bb[0] + row[80];
-      part[L.g_b1 + G.r] += bb[1] + row[81];
-    }
-  }
-  group_sync(G.g);                               // the scratch is the next step's H1 planes
-  G.fresh = 1u;
-  TL(G, 25);
+  for (int f = 0; f < 16; ++f) dx[f] = v[f];
 }
 
 }  // namespace tc2
 
 // ---------------------------------------------------------------------------------------------------------------
-// The kernel.  grid = min(#SM, ceil(#sub-tiles / 2)) CTAs of 512 threads, one CTA per SM (TMEM: 512 columns).
-// Slot s = 2 * blockIdx.x + group owns the contiguous sub-tile range [NSUB s / slots, NSUB (s + 1) / slots).
+// The kernel.  grid = min(#SM, #sub-tiles) CTAs of 256 threads, one CTA per SM (shared memory).
+// Slot s = NG * blockIdx.x + group owns the contiguous sub-tile range [NSUB s / slots, NSUB (s + 1) / slots).
 // INFADP swaps weight blobs (policy <-> v_target <-> v) through the one staging buffer: those swap points are CTA-wide
-// barriers, so both groups run the same number of (possibly empty) sub-tile iterations; FHADP groups never meet.
+// barriers, so with NG > 1 all groups run the same number of (possibly empty) sub-tile iterations.
 // ---------------------------------------------------------------------------------------------------------------
 template <class M, int ALG, int AF = -1>
 __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_constant__ KParams p) {
   using namespace tc2;
-  static_assert(M::KIND == 0, "tcgen05 rollout kernel: state == obs models");
+  static_assert(M::KIND == 0, "wgmma rollout kernel: state == obs models");
   constexpr int NS = M::NS, alg = ALG;
   extern __shared__ __align__(16) float smem[];
   unsigned char* sm = reinterpret_cast<unsigned char*>(smem);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sm);           // [0] weights, [1 + 4 g ..] group g: bc, bd2, bd1, bdx
-  uint32_t* tslot = reinterpret_cast<uint32_t*>(sm + 128);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sm);           // [0] weights landed
   float* Wsm = reinterpret_cast<float*>(sm + HDR_BYTES);
   unsigned char* ones = sm + HDR_BYTES + (size_t)p.w_floats * 4;
   unsigned char* gbase = ones + tcf::ONES_B;
 
   const int tid = threadIdx.x;
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);      // warp-uniform by construction (uniform-register MMA issue)
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);      // warp-uniform by construction
   Grp G;
   G.g = warp >> 3;
   G.wg = warp & 7;
@@ -643,34 +510,19 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
   G.Xp = G.Q + Q_BYTES;
   G.zp = reinterpret_cast<float*>(G.Xp + XP_BYTES);
   G.zb = G.zp + GT * MAXA;
+  G.A = reinterpret_cast<float*>(G.Xp + XP_BYTES + XCH_BYTES);
+  G.D1 = G.A + GT * AS;
+  G.DX = G.D1 + GT * AS;
   G.ones = ones;
-  G.bc = bars + 1 + 4 * G.g; G.bd2 = G.bc + 1; G.bd1 = G.bc + 2; G.bdx = G.bc + 3;
-  G.pc = G.pd2 = G.pd1 = G.pdx = 0u;
-  G.fresh = 1u;
-  G.d2_pending = G.d1_pending = false;
   const bool own = G.h == 0;
-#ifdef GOPS_TC2_TIMELINE
-  G.dbg = nullptr;
-  G.dbgn = 0;
-  if (p.dbg != nullptr && blockIdx.x == 0 && (tid == 0 || tid == 128)) G.dbg = p.dbg + (tid == 0 ? 0 : 4096);
-#endif
 
   if (tid == 0) {
-    for (int i = 0; i < 1 + 4 * NG; ++i) mbar_init(bars + i, 1);
+    mbar_init(bars, 1);
     fence_mbar_init();
   }
   if (tid < 256) {  // `ones`: [2 mn-groups][16 rows][8 bf16], feature 0 = 1.0
     uint16_t* o16 = reinterpret_cast<uint16_t*>(ones);
     o16[tid] = (tid < 128 && (tid & 7) == 0) ? (uint16_t)0x3f80 : (uint16_t)0;
-  }
-  if (warp == 0) umma::tmem_alloc(tslot, 512);
-  umma::fence_before_sync();
-  __syncthreads();
-  umma::fence_after_sync();
-  {
-    const uint32_t base = __shfl_sync(0xffffffffu, *tslot, 0);
-    G.tmg = base + C_GROUP * G.g;
-    G.tm = G.tmg + ((uint32_t)(32 * (G.wg & 3)) << 16);
   }
   uint32_t wphase = 0;
   auto stage = [&](const float* gsrc, int floats) {      // CTA-wide: both groups call it at the same program points
@@ -709,7 +561,7 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
   const long long s0 = nsub * slot / slots, s1 = nsub * (slot + 1) / slots;
   // INFADP: equal iteration counts for both groups of the CTA (stage() is a CTA-wide barrier)
   long long iters = s1 - s0;
-  if (alg == ALG_PIM || alg == ALG_PEV) {
+  if (NG > 1 && (alg == ALG_PIM || alg == ALG_PEV)) {
     const long long o0 = nsub * (slot ^ 1) / slots, o1 = nsub * ((slot ^ 1) + 1) / slots;
     iters = (o1 - o0) > iters ? (o1 - o0) : iters;
   }
@@ -739,7 +591,6 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
         layer1_issue<NS>(G, P, st, (float)(k + 1));
         layer1_finish<false, AF>(G, P, 2 * G.h, 2 * G.h + 2);
         layer2_out<AF>(G, P, z);
-        TL(G, 30);
         if (own) {
           float a[MAXA], g[MAXA], apol[MAXA];
           if (alg == ALG_FHADP || alg == ALG_PIM) {
@@ -807,7 +658,8 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           layer1_issue<NS>(G, V, st, 0.f);
           layer1_finish<true, AF>(G, V, 2 * G.h, 2 * G.h + 2);
           layer2_back<false, true, AF>(G, V, zb, zv, acc3);
-          backprop<false>(G, V, true, dx);
+          backprop<false>(G, V, true, part);
+          collect_dx(G, dx);
           if (term) {
 #pragma unroll
             for (int f = 0; f < NS; ++f)
@@ -830,7 +682,7 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
         float o0[NS];
 #pragma unroll
         for (int f = 0; f < NS; ++f) o0[f] = (own && valid && f < obs_dim) ? p.obs[gs * obs_dim + f] : 0.f;
-        float zv[MAXA], zb[MAXA], dx[16];
+        float zv[MAXA], zb[MAXA];
 #pragma unroll
         for (int j = 0; j < MAXA; ++j) zb[j] = zv[j] = 0.f;
         // the output adjoint needs v(o_0) first: forward to the output, then recompute layer 2 fused with the backward
@@ -844,8 +696,7 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           zb[0] = 2.f * diff * p.inv_B;
         }
         layer2_back<true, false, AF>(G, V, zb, nullptr, acc3);
-        backprop<true>(G, V, false, dx);
-        flush(G, V, part);
+        backprop<true>(G, V, false, part);
       }
       stage(p.blob_pol, P.blob);
       bind(G, Wsm, P);
@@ -881,8 +732,8 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
         for (int j = 0; j < MAXA; ++j)
           if (j < P.out) zt[j] = tape[(k * TCH + NS + 1 + j) * GT + G.r];
       }
-      layer1_issue<NS>(G, P, st, (float)(k + 1));     // recompute: issued first, the adjoint below overlaps the MMA
-      if (own && dx_pending) {                        // input gradient of step k + 1 (its MMAs ran under the code above)
+      layer1_issue<NS>(G, P, st, (float)(k + 1));     // recompute of step k's layer 1
+      if (own && dx_pending) {                        // input gradient of step k + 1
         float dxn[16];
         collect_dx(G, dxn);
         if (dx_add) {
@@ -895,7 +746,6 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
 #pragma unroll
       for (int j = 0; j < MAXA; ++j) zb[j] = 0.f;
       const bool active = own && valid && (p.mask_at_done ? !dnk : true);
-      TL(G, 31);
       if (own) {
         if (k > 0) {
 #pragma unroll
@@ -954,20 +804,15 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           for (int j = 0; j < MAXA; ++j) zb[j] = abar[j] * g[j];
         }
       }
-      TL(G, 32);
       layer1_finish<true, AF>(G, P, 0, G.h == 0 ? 0 : 4);      // the helper converts the whole row meanwhile
-      float dx[16];
       layer2_back<true, false, AF>(G, P, zb, nullptr, acc3);
-      backprop<true>(G, P, k > 0, dx, true);
+      backprop<true>(G, P, k > 0, part);
       dx_pending = k > 0;
       dx_add = active && k > 0;
-      if ((H - k) % FLUSH_EVERY == 0 || k == 0) flush(G, P, part);
     }
   }
 
   // ============================ per-group partials ============================
-  tc2::wait_d2(G);
-  tc2::wait_d1(G);
   group_sync(G.g);
   if (alg != ALG_TRACE) {
     const NetL& U = (alg == ALG_PEV) ? V : P;
@@ -1009,12 +854,6 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
       part[nparam + G.r] = s;
     }
   }
-#ifdef GOPS_TC2_TIMELINE
-  if (G.dbg != nullptr) G.dbg[4095] = G.dbgn;
-#endif
-  umma::fence_before_sync();
-  __syncthreads();
-  if (warp == 0) umma::tmem_dealloc(__shfl_sync(0xffffffffu, *tslot, 0), 512);
 }
 
 }  // namespace gops

@@ -1,0 +1,113 @@
+// Hopper (sm_90a) warpgroup tensor-core primitives: shared-memory matrix descriptors, wgmma.mma_async issue for BF16
+// (m64nNk16, N = 16 / 32 / 64 / 128) and TF32 (m64n64k8) with FP32 register accumulators, the fence / commit / wait of
+// the async group, and the fp32 -> TF32 hi / lo split.
+//
+// Operand layout used throughout: the no-swizzle canonical layout, core matrix = 8 rows x 16 bytes.
+//   plane[kc][r][16 B]   r = 0..R-1 rows, kc = 16-byte column chunk
+// core matrix (r/8, kc) starts at byte  kc * (R*16) + (r/8) * 128.
+//   K-major view  (M/N = r, K along the chunks):  LBO = R*16 (next K core matrix), SBO = 128 (next 8 rows)
+//   MN-major view (M/N along the chunks, K = r):  LBO = 128 (next 8 K rows),      SBO = R*16 (next 8 M/N columns)
+// so one buffer serves X.W^T (activations K-major) and, transposed, the weight-gradient contraction over samples
+// (MN-major operands exist for 16-bit types only).
+//
+// Accumulator fragment of m64nN (thread t of the warpgroup, w = t / 32, l = t % 32), register i in [0, N/2):
+//   row = 16 w + l / 4 + 8 ((i >> 1) & 1),  column = 8 (i >> 2) + 2 (l % 4) + (i & 1)
+#pragma once
+#include "common.cuh"
+
+namespace gops {
+namespace wg {
+
+// 64-bit wgmma shared-memory descriptor, no swizzle: start address, leading / stride byte offsets (all >> 4)
+__device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  return (uint64_t)((saddr >> 4) & 0x3fffu) | ((uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16) |
+         ((uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32);
+}
+
+// before the first wgmma that reads / writes accumulator registers the thread touched
+__device__ __forceinline__ void fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int PENDING>
+__device__ __forceinline__ void wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an async wgmma window
+template <int N>
+__device__ __forceinline__ void reg_fence(float* d) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D (+)= A . B^T on one warpgroup: M = 64 rows, K = 16 (bf16) or 8 (tf32).  acc = 0: D is overwritten.
+// TA / TB: 0 = K-major operand, 1 = MN-major (transposed) operand.
+template <int TA, int TB>
+__device__ __forceinline__ void mma_bf16_n16(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB)
+      : "memory");
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void mma_bf16_n32(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB)
+      : "memory");
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void mma_bf16_n64(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB)
+      : "memory");
+}
+
+template <int TA, int TB>
+__device__ __forceinline__ void mma_bf16_n128(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB)
+      : "memory");
+}
+
+__device__ __forceinline__ void mma_tf32_n64(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(acc)
+      : "memory");
+}
+
+template <int N, int TA, int TB>
+__device__ __forceinline__ void mma_bf16(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  static_assert(N == 16 || N == 32 || N == 64 || N == 128, "wgmma bf16 tile width");
+  if constexpr (N == 16) mma_bf16_n16<TA, TB>(d, a, b, acc);
+  else if constexpr (N == 32) mma_bf16_n32<TA, TB>(d, a, b, acc);
+  else if constexpr (N == 64) mma_bf16_n64<TA, TB>(d, a, b, acc);
+  else mma_bf16_n128<TA, TB>(d, a, b, acc);
+}
+
+// accumulator fragment coordinates (see the header comment)
+__device__ __forceinline__ int frag_row(int t, int i) { return 16 * (t >> 5) + ((t & 31) >> 2) + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int frag_col(int t, int i) { return 8 * (i >> 2) + 2 * (t & 3) + (i & 1); }
+
+// x = hi + lo exactly, hi on the TF32 grid (round to nearest, ties away); the tensor core truncates lo
+__device__ __forceinline__ void split(float x, float& hi, float& lo) {
+  hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
+  lo = x - hi;
+}
+
+// 128-thread named barrier of one warpgroup (ids 1..; id 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int g) { asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory"); }
+
+}  // namespace wg
+}  // namespace gops

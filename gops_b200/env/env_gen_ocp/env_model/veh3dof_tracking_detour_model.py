@@ -5,7 +5,7 @@ surrounding vehicle's ego-frame pose and speed (:62-76), other reward weights an
 info["constraint"] = 2 r - min distance of the bicircle collision model of the incoming state (:78-131) -- the constraint
 provider of FHADPExterior / FHADPLagrangian / FHADPInterior.  ContextState.constraint holds the surrounding vehicle's
 predictions [B, pre_horizon + 1, 1, 5] = (x, y, phi, u, delta) (context/ref_traj_with_static_obstacle.py:119-127).
-Kernels: csrc/lw_detour.cuh (the fused update on the layer-wise tcgen05 path; `forward` = veh_step_detour_kernel)."""
+Kernels: csrc/lw_detour.cuh (the fused update on the layer-wise wgmma path; `forward` = veh_step_detour_kernel)."""
 import math
 from typing import Union
 

@@ -1,4 +1,4 @@
-"""Host-side handle of the layer-wise tcgen05 MLP (C ABI `gops_b200_mlpnet_*`, csrc/dense_tc.cu): forward / backward of an
+"""Host-side handle of the layer-wise wgmma MLP (C ABI `gops_b200_mlpnet_*`, csrc/dense_tc.cu): forward / backward of an
 `mlp()` network (reference gops/apprfunc/mlp.py:36-41) of any depth with widths <= 256, evaluated on the tensor cores in
 BF16x3 (FP32-accurate) arithmetic.  Plumbing only: device buffers are torch tensors, the arithmetic is in the library."""
 import ctypes as C

@@ -1,5 +1,5 @@
 /*
- * gops_b200.h -- C ABI of libgops_b200.so: the B200 (sm_100a) implementation of GOPS's batched
+ * gops_b200.h -- C ABI of libgops_b200.so: the H100 (sm_90a) implementation of GOPS's batched
  * model-rollout + ADP-update hot path.
  *
  * The reference (GOPS) has no FFI: its boundary for this path is the Python plugin API
@@ -107,7 +107,7 @@ typedef struct gops_b200_plan_desc {
   gops_b200_reftraj reftraj;
   /* FHADP2 (gops/algorithm/fhadp2.py:98-121): open-loop policy.  1 = `policy` is a FiniteHorizonFullPolicy
    * (mlp.py:114-145): ONE evaluation on obs_0 emits all `horizon` actions, policy.out_dim = act_dim * horizon (<= 256),
-   * no time input; alg must be GOPS_ALG_FHADP.  Runs on the layer-wise tcgen05 path. */
+   * no time input; alg must be GOPS_ALG_FHADP.  Runs on the layer-wise wgmma path. */
   int32_t open_loop;
   /* pyth_veh3dofconti_errcstr (env_ocp/env_model/pyth_veh3dofconti_errcstr_model.py:19-55): the vehicle model that also
    * returns info["constraint"] = (|y_err| - y_error_tol, |u_err| - u_error_tol) of the incoming observation. */
@@ -116,7 +116,7 @@ typedef struct gops_b200_plan_desc {
   /* env_gen_ocp veh3dof_tracking_detour (1; env_gen_ocp/env_model/veh3dof_tracking_detour_model.py:13-176) or
    * veh3dof_tracking_surrcstr (2; veh3dof_tracking_surrcstr_model.py:13-181): model must be GOPS_MODEL_VEH3DOF_TRACKING;
    * obs_dim = 6 + 4 P + 4 (one surrounding vehicle), info["constraint"] = the bicircle collision constraint of the
-   * incoming state.  FHADP and its constrained variants, on the layer-wise tcgen05 path. */
+   * incoming state.  FHADP and its constrained variants, on the layer-wise wgmma path. */
   int32_t veh_detour;
   float veh_length, veh_width;
 } gops_b200_plan_desc;
@@ -159,7 +159,7 @@ int gops_b200_plan_set_gamma(gops_b200_plan* plan, double gamma);
 int gops_b200_plan_enable_timing(gops_b200_plan* plan, int enable);
 int gops_b200_plan_last_kernel_ms(gops_b200_plan* plan, float* ms);
 int gops_b200_plan_launch_info(const gops_b200_plan* plan, int32_t* out4);
-/* Kernel path of the fused rollout.  AUTO (default) picks per launch: tcgen05 / TMEM (BF16x3) where the nets are
+/* Kernel path of the fused rollout.  AUTO (default) picks per launch: wgmma (BF16x3) where the nets are
  * 64-wide with <= 16 inputs, the mma.sync (3xTF32) / FFMA kernels elsewhere.  A plan option instead of an environment
  * switch so that a test can state AND assert which kernel ran (the env var GOPS_B200_ROLLOUT=tc|mma still overrides
  * for A/B runs from the shell).  last_path: path of the most recent rollout launch of this plan (GOPS_PATH_*). */
@@ -237,7 +237,7 @@ int gops_b200_rollout_trace(gops_b200_plan* plan, const gops_b200_batch* batch,
                             float* rew_out, float* done_out, void* stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
- * Layer-wise MLP on the tensor cores (tcgen05 / TMEM, BF16x3): a trainable `mlp()` network of 1..8 Linear layers with
+ * Layer-wise MLP on the tensor cores (wgmma, BF16x3): a trainable `mlp()` network of 1..8 Linear layers with
  * widths <= 256, one hidden activation and a linear output -- reference gops/apprfunc/mlp.py:36-41 evaluated and
  * differentiated layer by layer.  It is the path of the networks the fused rollout kernels do not cover:
  * [256,256] policies (FHADP veh3dof_tracking), the [256,256,256] nets of DSAC (mlp.py:149-221, 271-296) and the

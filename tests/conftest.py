@@ -25,7 +25,7 @@ def pytest_configure(config):
         torch.set_num_threads(min(8, _usable_cores()))   # GPU boxes report far more cpus than their quota
     except Exception:
         pass
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):

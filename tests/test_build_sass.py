@@ -1,6 +1,6 @@
-"""The built objects must contain the instructions the design claims (checked on the SASS of the sm_100a cubins, no GPU
-needed): tcgen05 tensor-core MMAs with TMEM loads / stores and commit barriers in the rollout and inference kernels,
-TF32 mma.sync in the mma path, TMA bulk copies for the weight staging."""
+"""The built objects must contain the instructions the design claims (checked on the SASS of the sm_90a cubins, no GPU
+needed): warpgroup tensor-core MMAs (wgmma) in the tensor-core rollout, layer-wise and inference kernels, TF32 mma.sync
+in the fused mma.sync rollout kernel, TMA bulk copies for the weight staging."""
 import os
 import shutil
 import subprocess
@@ -33,22 +33,23 @@ def _objects():
 
 
 def test_rollout_objects_carry_tcgen05_tma_and_tf32_mma():
-    c = _count(os.path.join(_objects(), "kernels_idp.o"),
-               ["UTCHMMA", "LDTM", "STTM", "UTCBAR", "HMMA.1688.F32.TF32", "UBLKCP", "SYNCS"])
-    assert c["UTCHMMA"] > 100, c          # tcgen05.mma (rollout_tc2: BF16x3 layer / delta / weight-gradient products)
-    assert c["LDTM"] > 10 and c["STTM"] >= 4, c  # tcgen05.ld / tcgen05.st (TMEM epilogues; act'(layer 1) parked in TMEM)
-    assert c["UTCBAR"] > 8, c             # tcgen05.commit -> mbarrier
+    """(Name kept from the Blackwell build: the tensor-core rollout kernel is now wgmma.)"""
+    c = _count(os.path.join(_objects(), "kernels_idp.o"), ["HGMMA", "WARPGROUP.DEPBAR", "HMMA.1688.F32.TF32", "UBLKCP", "SYNCS"])
+    assert c["HGMMA"] > 100, c            # wgmma (rollout_tc2: BF16x3 layer / delta / weight-gradient products)
+    assert c["WARPGROUP.DEPBAR"] > 8, c   # wgmma.wait_group
     assert c["HMMA.1688.F32.TF32"] > 100, c      # mma.sync 3xTF32 path
     assert c["UBLKCP"] > 4, c             # cp.async.bulk weight staging
+    assert c["SYNCS"] > 8, c              # mbarrier transaction counts / phase checks of the staging
 
 
 def test_layerwise_objects_carry_tcgen05():
-    """dense_tc.o: the forward / dgrad / wgrad GEMMs of the layer-wise path; kernels_vehtrack.o only hosts the per-step
-    kernels of C3 (its dense products run in dense_tc.o)."""
-    c = _count(os.path.join(_objects(), "dense_tc.o"), ["UTCHMMA", "LDTM", "UTCBAR", "UBLKCP"])
-    assert c["UTCHMMA"] >= 90 and c["LDTM"] >= 5 and c["UTCBAR"] >= 5 and c["UBLKCP"] >= 4, c
+    """dense_tc.o: the forward / dgrad / wgrad GEMMs of the layer-wise path (wgmma; name kept from the Blackwell build);
+    kernels_vehtrack.o only hosts the per-step kernels of C3 (its dense products run in dense_tc.o)."""
+    c = _count(os.path.join(_objects(), "dense_tc.o"), ["HGMMA", "WARPGROUP.DEPBAR", "UBLKCP"])
+    assert c["HGMMA"] >= 90 and c["WARPGROUP.DEPBAR"] >= 5 and c["UBLKCP"] >= 4, c
 
 
 def test_inference_object_carries_tcgen05():
-    c = _count(os.path.join(_objects(), "gops_b200.o"), ["UTCHMMA", "LDTM", "UTCBAR", "UBLKCP"])
-    assert c["UTCHMMA"] >= 18 and c["LDTM"] >= 2 and c["UTCBAR"] >= 2 and c["UBLKCP"] >= 2, c
+    """The 64-wide inference kernel (wgmma TF32; name kept from the Blackwell build)."""
+    c = _count(os.path.join(_objects(), "gops_b200.o"), ["HGMMA.64x64x8.F32.TF32", "WARPGROUP.DEPBAR", "UBLKCP"])
+    assert c["HGMMA.64x64x8.F32.TF32"] >= 18 and c["WARPGROUP.DEPBAR"] >= 2 and c["UBLKCP"] >= 2, c

@@ -1,6 +1,6 @@
 """env_gen_ocp veh3dof_tracking_detour (N3: the model of the reference's fhadp_mlp_veh3ddetour example) and its sibling
 veh3dof_tracking_surrcstr with FHADP and the
-constrained variants FHADPExterior / FHADPLagrangian / FHADPInterior on the layer-wise tcgen05 path (csrc/lw_detour.cuh):
+constrained variants FHADPExterior / FHADPLagrangian / FHADPInterior on the layer-wise wgmma path (csrc/lw_detour.cuh):
 against the unmodified reference's golden vectors (two consecutive updates) and against the fp64 oracle on a fresh
 ragged batch with done samples -- whose state keeps evolving behind the frozen observation and keeps paying the
 constraint -- for the 64-wide nets of the goldens and the [256, 256] nets of the reference's example."""

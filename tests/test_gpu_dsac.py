@@ -1,4 +1,4 @@
-"""DSAC on the layer-wise tcgen05 path (algorithm/dsac.py, csrc/dsac.cu, csrc/dense_tc.cu) against
+"""DSAC on the layer-wise wgmma path (algorithm/dsac.py, csrc/dsac.cu, csrc/dense_tc.cu) against
 (a) the unmodified reference: tests/golden/dsac_idp.npz -- four consecutive `local_update`s replaying the Gaussian noise the
     reference drew (eps_new / eps_next / z_next recorded by oracle/make_golden.py), scalars, gradients of q / policy /
     log_alpha, the Adam steps (delayed policy update), Polyak targets and the temperature;

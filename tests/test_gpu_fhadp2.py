@@ -1,5 +1,5 @@
 """FHADP2 / FiniteHorizonFullPolicy (open-loop policy, reference gops/algorithm/fhadp2.py, mlp.py:114-145) on the layer-wise
-tcgen05 path: loss and gradient against an fp64 PyTorch restatement built from the oracle's env model (the rollout uses
+wgmma path: loss and gradient against an fp64 PyTorch restatement built from the oracle's env model (the rollout uses
 the oracle's wrapped model step by step with the action sequence of ONE policy evaluation), the golden vectors of the
 unmodified reference (tests/golden/fhadp2_idp.npz), and `forward_all_policy` inference."""
 import numpy as np

@@ -1,10 +1,10 @@
 """Parity AT THE BASELINE SIZES, on the path the library picks by itself (no environment switch; the test asserts which
-kernel ran through the plan's launch record): fused sm_100a update vs. the fp32 CPU oracle evaluated in chunks.
+kernel ran through the plan's launch record): fused sm_90a update vs. the fp32 CPU oracle evaluated in chunks.
 
-  C1  FHADP pyth_idpendulum   H=30  B=2^18 and a ragged 200 003          (tcgen05 kernel, many chunks per CTA)
+  C1  FHADP pyth_idpendulum   H=30  B=2^18 and a ragged 200 003          (wgmma kernel, many chunks per CTA)
   C2  INFADP pyth_veh3dofconti P=10 n=10 B=4096, PEV and PIM             (mma.sync kernel, 46 inputs)
-  C3  FHADP veh3dof_tracking  P=H=60 [256,256] elu B=8192 (one GPU's shard of 65 536): layer-wise tcgen05 path
-  C5  INFADP pyth_lq s4a2     n=10  B=2^16 (PEV, PIM) and 2^20 (PIM)     (tcgen05 kernel)
+  C3  FHADP veh3dof_tracking  P=H=60 [256,256] elu B=8192 (one GPU's shard of 65 536): layer-wise wgmma path
+  C5  INFADP pyth_lq s4a2     n=10  B=2^16 (PEV, PIM) and 2^20 (PIM)     (wgmma kernel)
 
 Bars: loss 1e-4 relative, gradient 2e-4 relative L2 (1e-3 for pyth_veh3dofconti, see test_gpu_parity.py), number of
 samples done at the end of the rollout EQUAL.  The fp32 oracle is itself within 2e-6 / 1e-5 of the unmodified

@@ -1,4 +1,4 @@
-"""Layer-wise tcgen05 MLP (csrc/dense_tc.cu, BF16x3) against a plain PyTorch reference of the same network evaluated in
+"""Layer-wise wgmma MLP (csrc/dense_tc.cu, BF16x3) against a plain PyTorch reference of the same network evaluated in
 fp64: outputs, parameter gradients (torch flat order) and input gradients, ragged batches, widths that are not
 multiples of the tile sizes, gradient accumulation, several live forward passes (slots).
 Bars: outputs 4e-6 relative to the output scale (FP32-accurate six-term products; FP32 accumulation over up to 256

@@ -1,4 +1,4 @@
-"""GPU parity: the fused sm_100a path (through the plugin API -> ctypes -> C ABI) against
+"""GPU parity: the fused sm_90a path (through the plugin API -> ctypes -> C ABI) against
 (a) golden vectors produced by the unmodified reference and (b) the CPU oracle on fresh inputs.
 
 Tolerances (fp32 path, different summation order and a closed-form 3x3 solve instead of LU):
@@ -186,7 +186,7 @@ def _oracle_nets(alg, hidden_act, dtype):
     ("veh3dof_tracking", "FHADP", "elu", 250, 10),
     ("pyth_idpendulum", "FHADP", "gelu256", 300, 8),
     ("pyth_lq", "INFADP", "relu256", 200, 5),
-    ("pyth_lq", "FHADP", "elu256", 700, 12),              # layer-wise tcgen05 path (wide nets, FHADP)
+    ("pyth_lq", "FHADP", "elu256", 700, 12),              # layer-wise wgmma path (wide nets, FHADP)
     ("veh3dof_tracking", "FHADP", "gelu256", 300, 10),
 ])
 def test_against_oracle_fp64(env_id, algname, act, B, H):

@@ -1,5 +1,5 @@
 """INTEGRATION.md's binding executed INSIDE the real reference: `gops.create_pkg.create_alg.register` swaps the fused
-B200 algorithm into the reference's registry, the reference's own factory builds it, the reference's own ReplayBuffer
+gops_b200 algorithm into the reference's registry, the reference's own factory builds it, the reference's own ReplayBuffer
 (gops/trainer/buffer/replay_buffer.py) feeds it, and three OffSerialTrainer-style steps (off_serial_trainer.py:79-105:
 sample_batch -> .cuda() -> alg.local_update) run next to the unmodified reference algorithm on the same batches.
 Needs the reference tree (oracle/_ref on the GPU box, oracle/build_ref.py)."""

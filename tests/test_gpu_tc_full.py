@@ -1,5 +1,5 @@
-"""Full tcgen05 rollout kernel (BF16x3 operands, TMEM weight-gradient accumulators; plan option kernel_path = "tc";
-csrc/mlp_tc_full.cuh) held to the same bars as the mma.sync kernel: golden vectors of the unmodified reference (loss,
+"""wgmma rollout kernel (BF16x3 operands, FP32 weight-gradient accumulation; plan option kernel_path = "tc";
+csrc/rollout_tc2.cuh) held to the same bars as the mma.sync kernel: golden vectors of the unmodified reference (loss,
 gradient, Adam step), the fp64 oracle on ragged batches, degenerate shapes and the no-grad trace."""
 import numpy as np
 import pytest
@@ -16,7 +16,7 @@ TC_GOLDEN = [n for n in base.GOLDEN
 
 @pytest.fixture(autouse=True)
 def _force_tc(monkeypatch):
-    """Every algorithm built in these tests asks its plans for the tcgen05 kernel (a plan option, asserted below)."""
+    """Every algorithm built in these tests asks its plans for the wgmma kernel (a plan option, asserted below)."""
     from gops_b200.algorithm.base import FusedADPMixin
     monkeypatch.setattr(FusedADPMixin, "kernel_path", "tc")
 
@@ -48,7 +48,7 @@ def test_tcf_trace_matches_reference_rollout():
 
 
 def test_tcf_path_is_taken_and_deterministic(monkeypatch):
-    """Same inputs: hybrid and mma.sync gradients agree to tolerance but not bitwise (the tcgen05 forward rounds
+    """Same inputs: hybrid and mma.sync gradients agree to tolerance but not bitwise (the wgmma forward rounds
     differently), and the hybrid path reproduces itself bit for bit."""
     alg, rec = base.build_alg("fhadp_idp_h30")
     data = base.data_from(rec, "pyth_idpendulum")

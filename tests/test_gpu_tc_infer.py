@@ -1,4 +1,4 @@
-"""tcgen05 / TMEM inference path (gops_b200/csrc/mlp_tc.cuh) against a float64 torch evaluation of the same
+"""wgmma inference path (gops_b200/csrc/mlp_tc.cuh) against a float64 torch evaluation of the same
 nn.Sequential (reference gops/apprfunc/mlp.py:73-77,103-111,327-329) and against the mma.sync path.
 Tolerance: 3xTF32 keeps ~2^-21 per product; outputs are O(1), so 5e-6 absolute / 1e-5 relative."""
 import copy

@@ -2,10 +2,11 @@
 
 * BF16x3 (csrc/mlp_tc_full.cuh): x = b0 + b1 + b2 with round-to-nearest bf16 planes leaves a residual <= 2^-24 |x|, and
   the six product terms of order <= 2 reproduce x*y to <= 2^-23 relative -- FP32-level, better than 3xTF32.
-* 3xTF32 (csrc/mma_tiles.cuh, umma.cuh): hi = round-to-nearest (ties away) onto the TF32 grid by integer add + mask,
+* 3xTF32 (csrc/mma_tiles.cuh, mlp_tc.cuh): hi = round-to-nearest (ties away) onto the TF32 grid by integer add + mask,
   lo = x - hi exact; hi*hi + hi*lo + lo*hi is within 2^-21 of x*y.
 * Truncating accumulation: adding N equal-sign terms into an FP32 accumulator with round-toward-zero loses ~N * 2^-25
-  relative -- the reason the TMEM-resident weight gradients are flushed every horizon step (DESIGN.md 3).
+  relative -- the reason the tensor-core weight gradients are added into an FP32 round-to-nearest partial every
+  horizon step (DESIGN.md 3).
 """
 import numpy as np
 import torch
@@ -87,9 +88,9 @@ def test_truncating_accumulation_bias_grows_with_chain_length():
 
 
 def test_bf16x3_mlp_forward_emulation_is_fp32_accurate():
-    """The full tcgen05 path's layer arithmetic emulated on the CPU (bf16x3 planes of activations and weights, six
+    """The wgmma rollout path's layer arithmetic emulated on the CPU (bf16x3 planes of activations and weights, six
     product terms, FP32-or-better accumulation): a 7 -> 64 -> 64 -> 1 gelu policy stays within 2e-6 of float64 --
-    the same margin the GPU parity tests measure (profiles/r01_parity_report.txt) -- while plain bf16 operands are
+    the same margin the GPU parity tests hold -- while plain bf16 operands are
     three orders of magnitude worse (SURVEY F8: why a split is needed at all)."""
     g = torch.Generator().manual_seed(3)
     B = 4096

@@ -1,5 +1,5 @@
 """Throughput of the batched policy inference (gops_b200_mlp_forward) on the two 64-wide CUDA paths:
-GOPS_B200_INFER=mma (mma.sync 3xTF32) vs tc (tcgen05 / TMEM 3xTF32).  Prints one JSON line per (mode, batch)."""
+GOPS_B200_INFER=mma (mma.sync 3xTF32) vs tc (wgmma 3xTF32).  Prints one JSON line per (mode, batch)."""
 import json
 import os
 import sys

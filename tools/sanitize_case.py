@@ -35,7 +35,7 @@ if "wide" in which:
     alg = create_alg(**kwargs("veh3dof_tracking", "FHADP", 46, 2, 256, "elu", pre_horizon=10))
     alg.set_parameters({"pre_horizon": 2})
     alg.local_update(sample("veh3dof_tracking", 70, 4, pre_horizon=10), 0)
-if "tc" in which:          # tcgen05 / TMEM kernels: hybrid rollout (forced) and batched inference incl. a ragged tail
+if "tc" in which:          # wgmma kernels: tensor-core rollout (forced) and batched inference incl. a ragged tail
     os.environ["GOPS_B200_ROLLOUT"] = "tc"
     alg = create_alg(**kwargs("pyth_idpendulum", "FHADP", 6, 1, 64, "gelu", pre_horizon=3, reward_scale=1.0))
     for B in (700, 130):
@@ -50,7 +50,7 @@ if "tc" in which:          # tcgen05 / TMEM kernels: hybrid rollout (forced) and
     alg.networks.policy(torch.randn(4321, 4, device="cuda"))
     alg.networks.v(torch.randn(129, 4, device="cuda"))
     os.environ.pop("GOPS_B200_INFER")
-if "lw" in which:          # layer-wise tcgen05 path: wide FHADP (C3 shape, small), FHADP2, a bare LayerwiseMlp with ragged shapes
+if "lw" in which:          # layer-wise wgmma path: wide FHADP (C3 shape, small), FHADP2, a bare LayerwiseMlp with ragged shapes
     alg = create_alg(**kwargs("veh3dof_tracking", "FHADP", 46, 2, 256, "elu", pre_horizon=10))
     alg.kernel_path = "tc"
     alg.set_parameters({"pre_horizon": 3})
