@@ -98,6 +98,11 @@ PROTOTYPES = {
                                            C.c_void_p, C.c_int32, C.c_void_p]),
     "gops_b200_mlpnet_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_void_p,
                                             C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]),
+    "gops_b200_mlpnet_pair_forward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_int32,
+                                                C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+    "gops_b200_mlpnet_pair_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64,
+                                                 C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                                 C.c_int32, C.c_void_p]),
     "gops_b200_mlpnet_keep_deltas": (C.c_int, [C.c_void_p, C.c_int32]),
     "gops_b200_mlpnet_wgrad_slots": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_int32,
                                                C.c_int64, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_int32,
@@ -112,6 +117,14 @@ PROTOTYPES = {
                                         C.c_int64, C.c_float, C.c_float, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gops_b200_dsac_policy_loss": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_float, C.c_void_p,
                                              C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gops_b200_dsact_q_loss": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_float, C.c_double,
+                                         C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gops_b200_dsact_policy_loss": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_float,
+                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gops_b200_dsact_sample_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_float,
+                                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_float,
+                                                  C.c_void_p, C.c_void_p]),
     "gops_b200_peer_create": (C.c_int, [C.c_int32, C.c_int32, C.c_int64, C.POINTER(C.c_void_p)]),
     "gops_b200_peer_destroy": (C.c_int, [C.c_void_p]),
     "gops_b200_peer_region_bytes": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),

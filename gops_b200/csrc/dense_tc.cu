@@ -1,6 +1,7 @@
 // C ABI of the generic wgmma dense-layer path (include/gops_b200.h, section "layer-wise MLP"): a trainable MLP of
 // any depth (widths <= 256 per layer) evaluated layer by layer with the kernels of dense_tc.cuh.  Used by the wide-net
-// FHADP path, DSAC and FHADP2; the fused rollout kernels remain the path for 64-wide nets with small inputs.
+// FHADP path, DSAC, DSAC-T (paired twin-critic passes) and FHADP2; the fused rollout kernels remain the path for 64-wide
+// nets with small inputs.
 #include "gops_b200.h"
 
 #include <cuda_bf16.h>
@@ -83,6 +84,182 @@ int launch_gemm(gops_b200_mlpnet* net, const dense::GemmArgs& a, cudaStream_t st
   gops::dense_count_launch(1);
   DCUDA(cudaGetLastError());
   (void)net;
+  return 0;
+}
+
+// One GEMM for `nn` networks of identical shape: the single-network kernel, or both networks of a pair in ONE launch
+// (blockIdx.z = network, same grid x / y and tiles as the single launch).
+template <int EPI, bool GRAD>
+int launch_gemm_n(gops_b200_mlpnet* const* nets, int nn, const dense::GemmArgs* a, cudaStream_t st) {
+  if (nn == 1) return launch_gemm<EPI, GRAD>(nets[0], a[0], st);
+  const size_t smem = dense::gemm_smem(a[0].n, GRAD);
+  static bool attr_of[64] = {};
+  bool& attr = attr_of[nets[0]->device & 63];
+  if (!attr) {
+    DCUDA(cudaFuncSetAttribute(dense::dense_gemm_pair_kernel<EPI, GRAD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)dense::gemm_smem(dense::NCMAX, GRAD)));
+    attr = true;
+  }
+  dense::GemmPair p;
+  p.g[0] = a[0];
+  p.g[1] = a[1];
+  dim3 grid((unsigned)((a[0].rows + dense::TM - 1) / dense::TM), (unsigned)dense::splits_of(a[0].n), 2u);
+  dense::dense_gemm_pair_kernel<EPI, GRAD><<<grid, dense::NTH, smem, st>>>(p);
+  gops::dense_count_launch(1);
+  DCUDA(cudaGetLastError());
+  return 0;
+}
+
+int set_wgrad_attr(gops_b200_mlpnet* const* nets, int nn) {
+  if (nn == 1) {
+    if (!nets[0]->attr_set) {
+      DCUDA(cudaFuncSetAttribute(dense::dense_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)dense::wgrad_smem()));
+      nets[0]->attr_set = true;
+    }
+    return 0;
+  }
+  static bool attr_of[64] = {};
+  bool& attr = attr_of[nets[0]->device & 63];
+  if (!attr) {
+    DCUDA(cudaFuncSetAttribute(dense::dense_wgrad_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)dense::wgrad_smem()));
+    attr = true;
+  }
+  return 0;
+}
+
+// Forward pass of `nn` (1 or 2) networks of identical shape on the same input x; network i writes y[i].
+int forward_n(gops_b200_mlpnet* const* nets, int nn, const float* x, int32_t ldx, int64_t batch, int32_t slot, int32_t train,
+              float* const* y, int32_t ldy, cudaStream_t st) {
+  for (int i = 0; i < nn; ++i) {
+    nets[i]->xin[slot] = x;
+    nets[i]->ldx[slot] = ldx;
+  }
+  const gops_b200_mlpnet* n0 = nets[0];
+  for (int l = 0; l < n0->nl; ++l) {
+    dense::GemmArgs a[2];
+    for (int i = 0; i < nn; ++i) {
+      gops_b200_mlpnet* net = nets[i];
+      memset(&a[i], 0, sizeof(a[i]));
+      a[i].A = l == 0 ? x : net->h[slot][l - 1];
+      a[i].lda = l == 0 ? ldx : net->sizes[l];
+      a[i].rows = batch;
+      a[i].k = net->sizes[l];
+      a[i].Bimg = net->fwd_img[l];
+      a[i].n = net->sizes[l + 1];
+      a[i].bias = net->params + net->b_off[l];
+      a[i].act = net->act;
+      if (l + 1 < net->nl) {
+        a[i].Y = net->h[slot][l]; a[i].ldy = a[i].n;
+        a[i].D = train ? net->d[slot][l] : nullptr; a[i].ldd = a[i].n;
+      } else {
+        a[i].Y = y[i]; a[i].ldy = ldy;
+      }
+    }
+    if (l + 1 < n0->nl) {
+      if (launch_gemm_n<dense::EPI_ACT, false>(nets, nn, a, st)) return 1;
+    } else {
+      if (launch_gemm_n<dense::EPI_LINEAR, false>(nets, nn, a, st)) return 1;
+    }
+  }
+  return 0;
+}
+
+// Backward pass of `nn` (1 or 2) networks of identical shape: network i takes dy[i] and writes grad[i] / dx[i]
+// (grad / dx are all NULL or all set).  Every weight-gradient contraction, column sum, reduction and dgrad GEMM is ONE
+// launch for all networks.
+int backward_n(gops_b200_mlpnet* const* nets, int nn, const float* const* dy, int32_t lddy, int64_t batch, int32_t slot,
+               float* const* grad, int32_t accumulate, float* const* dx, int32_t lddx, cudaStream_t st) {
+  if (set_wgrad_attr(nets, nn)) return 1;
+  const gops_b200_mlpnet* n0 = nets[0];
+  const float* delta[2] = {dy[0], nn > 1 ? dy[1] : nullptr};
+  int ldd = lddy;
+  for (int l = n0->nl - 1; l >= 0; --l) {
+    const int n = n0->sizes[l + 1], k = n0->sizes[l];
+    if (grad[0]) {
+      const int64_t tiles = (batch + dense::TM - 1) / dense::TM;
+      const int chunks = (int)(tiles < n0->wchunks ? tiles : n0->wchunks);
+      dense::WgradArgs w[2];
+      for (int i = 0; i < nn; ++i) {
+        const gops_b200_mlpnet* net = nets[i];
+        w[i].dY = delta[i]; w[i].ldy = ldd;
+        w[i].X = l == 0 ? net->xin[slot] : net->h[slot][l - 1]; w[i].ldx = l == 0 ? net->ldx[slot] : k;
+        w[i].rows = batch; w[i].n = n; w[i].k = k;
+        w[i].partial = net->wpart;
+        w[i].tiles_per_chunk = (int)((tiles + chunks - 1) / chunks);
+        w[i].nslots = 1; w[i].sy = 0; w[i].sx = 0;
+      }
+      const long long nk = (long long)n * k;
+      const int brows = 64;
+      const long long rpb = (batch + brows - 1) / brows;
+      const unsigned wblocks = (unsigned)(((n + 127) / 128) * ((k + 127) / 128));
+      if (nn == 1) {
+        gops_b200_mlpnet* net = nets[0];
+        dense::dense_wgrad_kernel<<<dim3(wblocks, (unsigned)chunks), dense::NTH, dense::wgrad_smem(), st>>>(w[0]);
+        dense::dense_reduce_kernel<<<(unsigned)((nk + 255) / 256), 256, 0, st>>>(net->wpart, chunks, nk,
+                                                                               grad[0] + net->w_off[l], accumulate);
+        dense::dense_colsum_kernel<<<dim3((unsigned)((n + 31) / 32), (unsigned)brows), dim3(32, 8), 0, st>>>(
+            delta[0], ldd, batch, n, net->bpart, rpb, 1, 0);
+        dense::dense_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(net->bpart, brows, n,
+                                                                              grad[0] + net->b_off[l], accumulate);
+      } else {
+        const gops_b200_mlpnet* a = nets[0];
+        const gops_b200_mlpnet* b = nets[1];
+        dense::WgradPair wp;
+        wp.g[0] = w[0];
+        wp.g[1] = w[1];
+        dense::dense_wgrad_pair_kernel<<<dim3(wblocks, (unsigned)chunks, 2u), dense::NTH, dense::wgrad_smem(), st>>>(wp);
+        dense::dense_reduce_pair_kernel<<<dim3((unsigned)((nk + 255) / 256), 1u, 2u), 256, 0, st>>>(
+            a->wpart, b->wpart, chunks, nk, grad[0] + a->w_off[l], grad[1] + b->w_off[l], accumulate);
+        dense::dense_colsum_pair_kernel<<<dim3((unsigned)((n + 31) / 32), (unsigned)brows, 2u), dim3(32, 8), 0, st>>>(
+            delta[0], delta[1], ldd, batch, n, a->bpart, b->bpart, rpb);
+        dense::dense_reduce_pair_kernel<<<dim3((unsigned)((n + 255) / 256), 1u, 2u), 256, 0, st>>>(
+            a->bpart, b->bpart, brows, n, grad[0] + a->b_off[l], grad[1] + b->b_off[l], accumulate);
+      }
+      gops::dense_count_launch(4);
+      DCUDA(cudaGetLastError());
+    }
+    if (l > 0 || dx[0]) {
+      dense::GemmArgs a[2];
+      float* outb[2] = {};
+      for (int i = 0; i < nn; ++i) {
+        gops_b200_mlpnet* net = nets[i];
+        memset(&a[i], 0, sizeof(a[i]));
+        a[i].A = delta[i]; a[i].lda = ldd; a[i].rows = batch; a[i].k = n;      // contraction over the layer's outputs
+        a[i].Bimg = net->bwd_img[l];
+        a[i].n = k;
+        if (l > 0) {
+          outb[i] = net->keep_deltas ? net->gl[slot][l - 1] : net->delta[(net->nl - l) & 1];
+          a[i].mul = net->d[slot][l - 1]; a[i].ldm = k;
+          a[i].Y = outb[i]; a[i].ldy = k;
+        } else {
+          a[i].Y = dx[i]; a[i].ldy = lddx;
+        }
+      }
+      if (l > 0) {
+        if (launch_gemm_n<dense::EPI_MUL, true>(nets, nn, a, st)) return 1;
+        for (int i = 0; i < nn; ++i) delta[i] = outb[i];
+        ldd = k;
+      } else {
+        if (launch_gemm_n<dense::EPI_PLAIN, true>(nets, nn, a, st)) return 1;
+      }
+    }
+  }
+  return 0;
+}
+
+// Two handles may run as a pair when their shapes, activation, max_batch and slots agree and both are packed on
+// the same device.
+int check_pair(const gops_b200_mlpnet* a, const gops_b200_mlpnet* b, const char* fn) {
+  if (!a || !b) return dense_fail(std::string(fn) + ": null network handle");
+  if (a == b) return dense_fail(std::string(fn) + ": the two networks of a pair must be distinct handles");
+  bool same = a->nl == b->nl && a->act == b->act && a->max_batch == b->max_batch && a->slots == b->slots &&
+              a->device == b->device;
+  for (int l = 0; same && l <= a->nl; ++l) same = a->sizes[l] == b->sizes[l];
+  if (!same)
+    return dense_fail(std::string(fn) + ": the two networks differ in layer sizes, activation, max_batch, slots or device");
+  if (!a->params || !b->params) return dense_fail(std::string(fn) + " before mlpnet_pack of both networks");
   return 0;
 }
 
@@ -177,30 +354,7 @@ int gops_b200_mlpnet_forward(gops_b200_mlpnet* net, const float* x, int32_t ldx,
   if (!net->params) return dense_fail("mlpnet_forward before mlpnet_pack");
   if (batch < 1 || batch > net->max_batch || slot < 0 || slot >= net->slots) return dense_fail("mlpnet_forward: bad batch / slot");
   DevGuard2 dg(net->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  net->xin[slot] = x;
-  net->ldx[slot] = ldx;
-  for (int l = 0; l < net->nl; ++l) {
-    dense::GemmArgs a;
-    memset(&a, 0, sizeof(a));
-    a.A = l == 0 ? x : net->h[slot][l - 1];
-    a.lda = l == 0 ? ldx : net->sizes[l];
-    a.rows = batch;
-    a.k = net->sizes[l];
-    a.Bimg = net->fwd_img[l];
-    a.n = net->sizes[l + 1];
-    a.bias = net->params + net->b_off[l];
-    a.act = net->act;
-    if (l + 1 < net->nl) {
-      a.Y = net->h[slot][l]; a.ldy = a.n;
-      a.D = train ? net->d[slot][l] : nullptr; a.ldd = a.n;
-      if (launch_gemm<dense::EPI_ACT, false>(net, a, st)) return 1;
-    } else {
-      a.Y = y; a.ldy = ldy;
-      if (launch_gemm<dense::EPI_LINEAR, false>(net, a, st)) return 1;
-    }
-  }
-  return 0;
+  return forward_n(&net, 1, x, ldx, batch, slot, train, &y, ldy, (cudaStream_t)stream);
 }
 
 int gops_b200_mlpnet_backward(gops_b200_mlpnet* net, const float* dy, int32_t lddy, int64_t batch, int32_t slot,
@@ -209,59 +363,37 @@ int gops_b200_mlpnet_backward(gops_b200_mlpnet* net, const float* dy, int32_t ld
   if (batch < 1 || batch > net->max_batch || slot < 0 || slot >= net->slots || !net->xin[slot])
     return dense_fail("mlpnet_backward: no forward pass recorded in this slot");
   DevGuard2 dg(net->device);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (!net->attr_set) {
-    DCUDA(cudaFuncSetAttribute(dense::dense_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dense::wgrad_smem()));
-    net->attr_set = true;
-  }
-  const float* delta = dy;
-  int ldd = lddy;
-  for (int l = net->nl - 1; l >= 0; --l) {
-    const int n = net->sizes[l + 1], k = net->sizes[l];
-    const float* in = l == 0 ? net->xin[slot] : net->h[slot][l - 1];
-    const int ldin = l == 0 ? net->ldx[slot] : k;
-    if (grad_flat) {
-      dense::WgradArgs w;
-      w.dY = delta; w.ldy = ldd; w.X = in; w.ldx = ldin; w.rows = batch; w.n = n; w.k = k;
-      w.partial = net->wpart;
-      const int64_t tiles = (batch + dense::TM - 1) / dense::TM;
-      const int chunks = (int)(tiles < net->wchunks ? tiles : net->wchunks);
-      w.tiles_per_chunk = (int)((tiles + chunks - 1) / chunks);
-      w.nslots = 1; w.sy = 0; w.sx = 0;
-      dim3 grid((unsigned)(((n + 127) / 128) * ((k + 127) / 128)), (unsigned)chunks);
-      dense::dense_wgrad_kernel<<<grid, dense::NTH, dense::wgrad_smem(), st>>>(w);
-      const long long nk = (long long)n * k;
-      dense::dense_reduce_kernel<<<(unsigned)((nk + 255) / 256), 256, 0, st>>>(net->wpart, chunks, nk, grad_flat + net->w_off[l],
-                                                                             accumulate);
-      const int brows = 64;
-      const long long rpb = (batch + brows - 1) / brows;
-      dense::dense_colsum_kernel<<<dim3((unsigned)((n + 31) / 32), (unsigned)brows), dim3(32, 8), 0, st>>>(delta, ldd, batch, n,
-                                                                                                     net->bpart, rpb, 1, 0);
-      dense::dense_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(net->bpart, brows, n, grad_flat + net->b_off[l],
-                                                                            accumulate);
-      gops::dense_count_launch(4);
-      DCUDA(cudaGetLastError());
-    }
-    if (l > 0 || dx) {
-      dense::GemmArgs a;
-      memset(&a, 0, sizeof(a));
-      a.A = delta; a.lda = ldd; a.rows = batch; a.k = n;      // contraction over the layer's outputs
-      a.Bimg = net->bwd_img[l];
-      a.n = k;
-      if (l > 0) {
-        float* outb = net->keep_deltas ? net->gl[slot][l - 1] : net->delta[(net->nl - l) & 1];
-        a.mul = net->d[slot][l - 1]; a.ldm = k;
-        a.Y = outb; a.ldy = k;
-        if (launch_gemm<dense::EPI_MUL, true>(net, a, st)) return 1;
-        delta = outb;
-        ldd = k;
-      } else {
-        a.Y = dx; a.ldy = lddx;
-        if (launch_gemm<dense::EPI_PLAIN, true>(net, a, st)) return 1;
-      }
-    }
-  }
-  return 0;
+  return backward_n(&net, 1, &dy, lddy, batch, slot, &grad_flat, accumulate, &dx, lddx, (cudaStream_t)stream);
+}
+
+int gops_b200_mlpnet_pair_forward(gops_b200_mlpnet* net_a, gops_b200_mlpnet* net_b, const float* x, int32_t ldx,
+                                  int64_t batch, int32_t slot, int32_t train, float* y_a, float* y_b, int32_t ldy,
+                                  void* stream) {
+  if (check_pair(net_a, net_b, "mlpnet_pair_forward")) return 1;
+  if (!x || !y_a || !y_b) return dense_fail("mlpnet_pair_forward: null argument");
+  if (batch < 1 || batch > net_a->max_batch || slot < 0 || slot >= net_a->slots)
+    return dense_fail("mlpnet_pair_forward: bad batch / slot");
+  DevGuard2 dg(net_a->device);
+  gops_b200_mlpnet* nets[2] = {net_a, net_b};
+  float* ys[2] = {y_a, y_b};
+  return forward_n(nets, 2, x, ldx, batch, slot, train, ys, ldy, (cudaStream_t)stream);
+}
+
+int gops_b200_mlpnet_pair_backward(gops_b200_mlpnet* net_a, gops_b200_mlpnet* net_b, const float* dy_a, const float* dy_b,
+                                   int32_t lddy, int64_t batch, int32_t slot, float* grad_a, float* grad_b,
+                                   int32_t accumulate, float* dx_a, float* dx_b, int32_t lddx, void* stream) {
+  if (check_pair(net_a, net_b, "mlpnet_pair_backward")) return 1;
+  if (!dy_a || !dy_b) return dense_fail("mlpnet_pair_backward: null argument");
+  if (!grad_a != !grad_b || !dx_a != !dx_b)
+    return dense_fail("mlpnet_pair_backward: grad_a / grad_b and dx_a / dx_b must both be set or both be NULL");
+  if (batch < 1 || batch > net_a->max_batch || slot < 0 || slot >= net_a->slots || !net_a->xin[slot] || !net_b->xin[slot])
+    return dense_fail("mlpnet_pair_backward: no forward pass recorded in this slot");
+  DevGuard2 dg(net_a->device);
+  gops_b200_mlpnet* nets[2] = {net_a, net_b};
+  const float* dys[2] = {dy_a, dy_b};
+  float* grads[2] = {grad_a, grad_b};
+  float* dxs[2] = {dx_a, dx_b};
+  return backward_n(nets, 2, dys, lddy, batch, slot, grads, accumulate, dxs, lddx, (cudaStream_t)stream);
 }
 
 /* Keep the per-layer deltas of every backward pass in its slot (memory: slots x max_batch x width per hidden layer) so

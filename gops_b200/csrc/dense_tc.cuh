@@ -250,14 +250,30 @@ __device__ __forceinline__ void dense_gemm_body(const GemmArgs& g, unsigned char
 }
 
 template <int EPI, bool GRAD>
-__global__ void __launch_bounds__(NTH, 1) dense_gemm_kernel(const __grid_constant__ GemmArgs g) {
-  extern __shared__ __align__(128) unsigned char dsm[];
+__device__ __forceinline__ void dense_gemm_tile(const GemmArgs& g, unsigned char* dsm) {
   switch (nc_of(g.n)) {
     case 16: dense_gemm_body<EPI, GRAD, 16>(g, dsm); break;
     case 32: dense_gemm_body<EPI, GRAD, 32>(g, dsm); break;
     case 64: dense_gemm_body<EPI, GRAD, 64>(g, dsm); break;
     default: dense_gemm_body<EPI, GRAD, 128>(g, dsm); break;
   }
+}
+
+template <int EPI, bool GRAD>
+__global__ void __launch_bounds__(NTH, 1) dense_gemm_kernel(const __grid_constant__ GemmArgs g) {
+  extern __shared__ __align__(128) unsigned char dsm[];
+  dense_gemm_tile<EPI, GRAD>(g, dsm);
+}
+
+// Two networks of identical shape in one launch (twin critics): blockIdx.z selects the network, every CTA of network z
+// computes exactly the tile the single-network kernel computes for it.
+struct GemmPair {
+  GemmArgs g[2];
+};
+template <int EPI, bool GRAD>
+__global__ void __launch_bounds__(NTH, 1) dense_gemm_pair_kernel(const __grid_constant__ GemmPair p) {
+  extern __shared__ __align__(128) unsigned char dsm[];
+  dense_gemm_tile<EPI, GRAD>(p.g[blockIdx.z], dsm);
 }
 
 inline size_t gemm_smem(int n, bool grad) { return 128 + 2 * ((size_t)(grad ? 2 : 3) * 8 * TM * 16 + slice_bytes(nc_of(n))); }
@@ -336,8 +352,7 @@ __device__ __forceinline__ void dense_wgrad_body(const WgradArgs& g, unsigned ch
 }
 
 // dW partial of one (128 output features, <= 128 input features) block over a chunk of the rows
-__global__ void __launch_bounds__(NTH, 1) dense_wgrad_kernel(const __grid_constant__ WgradArgs g) {
-  extern __shared__ __align__(128) unsigned char dsm[];
+__device__ __forceinline__ void dense_wgrad_block(const WgradArgs& g, unsigned char* dsm) {
   const int kb = (g.k + 127) / 128, nb_i = blockIdx.x / kb, kb_i = blockIdx.x % kb;
   const int n0 = nb_i * 128, k0 = kb_i * 128;
   const int kw = (g.k - k0) < 128 ? (g.k - k0) : 128;                   // input features of this block
@@ -346,22 +361,42 @@ __global__ void __launch_bounds__(NTH, 1) dense_wgrad_kernel(const __grid_consta
   else if (kw <= 64) dense_wgrad_body<64>(g, dsm, n0, k0);
   else dense_wgrad_body<128>(g, dsm, n0, k0);
 }
+__global__ void __launch_bounds__(NTH, 1) dense_wgrad_kernel(const __grid_constant__ WgradArgs g) {
+  extern __shared__ __align__(128) unsigned char dsm[];
+  dense_wgrad_block(g, dsm);
+}
+struct WgradPair {
+  WgradArgs g[2];
+};
+__global__ void __launch_bounds__(NTH, 1) dense_wgrad_pair_kernel(const __grid_constant__ WgradPair p) {
+  extern __shared__ __align__(128) unsigned char dsm[];
+  dense_wgrad_block(p.g[blockIdx.z], dsm);
+}
 inline size_t wgrad_smem() { return 128 + (size_t)4 * 16 * TM * 16; }
 
 // grad[i] (+)= sum_c partial[c][i] in fixed chunk order
-__global__ void dense_reduce_kernel(const float* __restrict__ partial, int chunks, long long n, float* __restrict__ grad,
-                                    int accumulate) {
+__device__ __forceinline__ void dense_reduce_elem(const float* __restrict__ partial, int chunks, long long n,
+                                                  float* __restrict__ grad, int accumulate) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   float s = 0.f;
   for (int c = 0; c < chunks; ++c) s += partial[(size_t)c * n + i];
   grad[i] = accumulate ? grad[i] + s : s;
 }
+__global__ void dense_reduce_kernel(const float* __restrict__ partial, int chunks, long long n, float* __restrict__ grad,
+                                    int accumulate) {
+  dense_reduce_elem(partial, chunks, n, grad, accumulate);
+}
+// the same for two networks (blockIdx.z)
+__global__ void dense_reduce_pair_kernel(const float* __restrict__ partial0, const float* __restrict__ partial1, int chunks,
+                                         long long n, float* __restrict__ grad0, float* __restrict__ grad1, int accumulate) {
+  dense_reduce_elem(blockIdx.z ? partial1 : partial0, chunks, n, blockIdx.z ? grad1 : grad0, accumulate);
+}
 // db[n] (+)= sum_r dY[r][n]: one warp per (column, row chunk) pair would be the fast way; the layer widths here are
 // <= 256 and this is 0.1 % of the update, so: block = 32 columns x 8 row-lanes, fixed-order tree, partials per block row
-__global__ void dense_colsum_kernel(const float* __restrict__ dY, int ld, long long rows, int n, float* __restrict__ partial,
-                                    long long rows_per_block, int nslots, long long sy) {
-  __shared__ float sm[8][33];
+__device__ __forceinline__ void dense_colsum_block(const float* __restrict__ dY, int ld, long long rows, int n,
+                                                   float* __restrict__ partial, long long rows_per_block, int nslots,
+                                                   long long sy, float (*sm)[33]) {
   const int c = blockIdx.x * 32 + threadIdx.x, ry = threadIdx.y;
   const long long r0 = (long long)blockIdx.y * rows_per_block;
   const long long r1 = r0 + rows_per_block < rows ? r0 + rows_per_block : rows;
@@ -379,6 +414,18 @@ __global__ void dense_colsum_kernel(const float* __restrict__ dY, int ld, long l
     for (int j = 0; j < 8; ++j) t += sm[j][threadIdx.x];
     partial[(size_t)blockIdx.y * n + c] = t;
   }
+}
+__global__ void dense_colsum_kernel(const float* __restrict__ dY, int ld, long long rows, int n, float* __restrict__ partial,
+                                    long long rows_per_block, int nslots, long long sy) {
+  __shared__ float sm[8][33];
+  dense_colsum_block(dY, ld, rows, n, partial, rows_per_block, nslots, sy, sm);
+}
+// the same for two networks (blockIdx.z); both read `ld` floats per row of their dY
+__global__ void dense_colsum_pair_kernel(const float* __restrict__ dY0, const float* __restrict__ dY1, int ld, long long rows,
+                                         int n, float* __restrict__ partial0, float* __restrict__ partial1,
+                                         long long rows_per_block) {
+  __shared__ float sm[8][33];
+  dense_colsum_block(blockIdx.z ? dY1 : dY0, ld, rows, n, blockIdx.z ? partial1 : partial0, rows_per_block, 1, 0, sm);
 }
 
 }  // namespace dense

@@ -10,6 +10,8 @@
 
 #include <string>
 
+#include "dsac_common.cuh"
+
 namespace gops {
 int dense_fail(const std::string& msg);
 void dense_count_launch(int n);
@@ -17,8 +19,7 @@ void dense_count_launch(int n);
 
 namespace {
 
-constexpr float kEps = 1e-6f;                    // act_distribution_type.py:15 EPS
-constexpr float kHalfLog2Pi = 0.91893853320467274178f;
+using namespace gops::dsac;
 
 struct DevGuard3 {
   int prev = -1;
@@ -71,38 +72,7 @@ __global__ void dsac_sample_bwd_kernel(const float* __restrict__ logits, const f
                                        int ldda, int a0, float c, float* __restrict__ dlogits) {
   const long long b = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= B) return;
-  for (int j = 0; j < A; ++j) {
-    const float mean = logits[b * 2 * A + j], raw = logits[b * 2 * A + A + j];
-    const float ls = fminf(fmaxf(raw, lo), hi), sd = expf(ls), e = eps[b * A + j];
-    const float u = mean + sd * e, t = tanhf(u), om = 1.f - t * t;
-    // act = half t + mid;   -log(1 + EPS - t^2) has derivative 2 t (1 - t^2) / (1 + EPS - t^2) w.r.t. u
-    const float du = dA[b * ldda + a0 + j] * half[j] * om + c * (2.f * t * om / (1.f + kEps - t * t));
-    const float dls = (du * e * sd - c) * ((raw >= lo && raw <= hi) ? 1.f : 0.f);   // d(-log std)/d ls = -1
-    dlogits[b * 2 * A + j] = du;
-    dlogits[b * 2 * A + A + j] = dls;
-  }
-}
-
-// q head of ActionValueDistri (mlp.py:289-296): mean | softplus(raw)
-__device__ __forceinline__ float softplus(float x) { return x > 20.f ? x : log1pf(expf(x)); }   // torch threshold 20
-__device__ __forceinline__ float sigmoidf(float x) { return 1.f / (1.f + expf(-x)); }
-
-// column sums in fixed order: out[c] = sum_b f_c(b); one block per column-block, sequential over a strided range then
-// a fixed tree.  Used for the batch means below.
-template <class F>
-__device__ float block_sum(long long B, F f) {
-  __shared__ float sm[256];
-  float s = 0.f;
-  for (long long i = threadIdx.x; i < B; i += 256) s += f(i);
-  sm[threadIdx.x] = s;
-  __syncthreads();
-  for (int o = 128; o > 0; o >>= 1) {
-    if (threadIdx.x < o) sm[threadIdx.x] += sm[threadIdx.x + o];
-    __syncthreads();
-  }
-  const float r = sm[0];
-  __syncthreads();
-  return r;
+  sample_bwd_row(logits, eps, b, A, lo, hi, half, c, [&](int j) { return dA[b * ldda + a0 + j]; }, dlogits);
 }
 
 // Critic loss (dsac.py:219-262, bound = True):

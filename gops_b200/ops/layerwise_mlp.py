@@ -56,3 +56,42 @@ class LayerwiseMlp:
                 self.handle, _lib.ptr(dy), dy.stride(0), B, slot, _lib.ptr(grad), int(accumulate), _lib.ptr(dx),
                 dx.stride(0) if dx is not None else 0, _lib.stream_ptr()))
         return dx
+
+
+class LayerwiseMlpPair:
+    """Two `LayerwiseMlp` handles of identical shape (twin critics) evaluated on one shared input with paired passes
+    (`gops_b200_mlpnet_pair_*`): every layer launch runs both networks, each with the arithmetic of its single pass."""
+
+    def __init__(self, a: LayerwiseMlp, b: LayerwiseMlp):
+        self.a, self.b = a, b
+        self.device = a.device
+
+    def forward(self, x: torch.Tensor, slot: int = 0, train: bool = True, out_a: Optional[torch.Tensor] = None,
+                out_b: Optional[torch.Tensor] = None):
+        assert x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and x.stride(1) == 1
+        B, n = x.shape[0], self.a.sizes[-1]
+        ya = out_a if out_a is not None else torch.empty((B, n), dtype=torch.float32, device=x.device)
+        yb = out_b if out_b is not None else torch.empty((B, n), dtype=torch.float32, device=x.device)
+        assert ya.stride(0) == yb.stride(0) and ya.stride(1) == 1 and yb.stride(1) == 1
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().gops_b200_mlpnet_pair_forward(
+                self.a.handle, self.b.handle, _lib.ptr(x), x.stride(0), B, slot, int(train), _lib.ptr(ya), _lib.ptr(yb),
+                ya.stride(0), _lib.stream_ptr()))
+        return ya, yb
+
+    def backward(self, dy_a: torch.Tensor, dy_b: torch.Tensor, slot: int = 0, grad_a: Optional[torch.Tensor] = None,
+                 grad_b: Optional[torch.Tensor] = None, accumulate: bool = False, want_dx: bool = False):
+        for dy in (dy_a, dy_b):
+            assert dy.is_cuda and dy.dtype == torch.float32 and dy.dim() == 2 and dy.stride(1) == 1
+        assert dy_a.shape == dy_b.shape and dy_a.stride(0) == dy_b.stride(0)
+        B = dy_a.shape[0]
+        dx_a = dx_b = None
+        if want_dx:
+            dx_a = torch.empty((B, self.a.sizes[0]), dtype=torch.float32, device=dy_a.device)
+            dx_b = torch.empty_like(dx_a)
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.lib().gops_b200_mlpnet_pair_backward(
+                self.a.handle, self.b.handle, _lib.ptr(dy_a), _lib.ptr(dy_b), dy_a.stride(0), B, slot, _lib.ptr(grad_a),
+                _lib.ptr(grad_b), int(accumulate), _lib.ptr(dx_a), _lib.ptr(dx_b),
+                dx_a.stride(0) if dx_a is not None else 0, _lib.stream_ptr()))
+        return dx_a, dx_b

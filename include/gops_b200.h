@@ -263,6 +263,19 @@ int gops_b200_mlpnet_backward(gops_b200_mlpnet* net, const float* dy, int32_t ld
  * (called with grad_flat = NULL) leave its per-layer deltas in its slot; wgrad_slots then contracts the weight
  * gradients over all `nslots` passes at once (x / dy: input and output adjoint of slot0; slot s of them starts
  * x_stride / dy_stride rows further). */
+/* Paired passes (twin critics): two handles created with identical sizes, activation, max_batch and slots, both packed,
+ * evaluated on ONE shared input x.  Every forward GEMM, dgrad GEMM, weight-gradient contraction, column sum and
+ * reduction runs both networks in one launch (blockIdx.z selects the network), so a pair issues as many launches as one
+ * single-network pass.  Per network the arithmetic is that of mlpnet_forward / mlpnet_backward (same tiles, same
+ * reduction order: bit-identical results); each network keeps its own activations in `slot`.  y_a / y_b share ldy,
+ * dy_a / dy_b share lddy, dx_a / dx_b share lddx; grad_a / grad_b and dx_a / dx_b are both set or both NULL.  A
+ * mismatched pair returns an error. */
+int gops_b200_mlpnet_pair_forward(gops_b200_mlpnet* net_a, gops_b200_mlpnet* net_b, const float* x, int32_t ldx,
+                                  int64_t batch, int32_t slot, int32_t train, float* y_a, float* y_b, int32_t ldy,
+                                  void* stream);
+int gops_b200_mlpnet_pair_backward(gops_b200_mlpnet* net_a, gops_b200_mlpnet* net_b, const float* dy_a, const float* dy_b,
+                                   int32_t lddy, int64_t batch, int32_t slot, float* grad_a, float* grad_b,
+                                   int32_t accumulate, float* dx_a, float* dx_b, int32_t lddx, void* stream);
 int gops_b200_mlpnet_keep_deltas(gops_b200_mlpnet* net, int32_t enable);
 int gops_b200_mlpnet_wgrad_slots(gops_b200_mlpnet* net, int32_t slot0, int32_t nslots, int64_t batch, const float* x,
                                  int32_t ldx, int64_t x_stride, const float* dy, int32_t lddy, int64_t dy_stride,
@@ -292,6 +305,33 @@ int gops_b200_dsac_q_loss(const float* q_out, const float* q_next_out, const flo
                           float* d_q_out, float* out3, void* stream);
 int gops_b200_dsac_policy_loss(const float* q_out, const float* logp_new, int64_t batch, float alpha,
                                float target_entropy, float* d_q_out, float* out5, const float* stats, void* stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * DSAC-T (gops/algorithm/dsact.py:162-329): the elementwise half of the twin-critic update.  The critic evaluations
+ * between them are gops_b200_mlpnet_pair_* calls; action sampling is gops_b200_dsac_sample.
+ *
+ * q_loss:   dsact.py:229-313.  q1_out / q2_out: critic outputs [B][2] (mean | raw std) at (obs, act); q1_next_out /
+ *           q2_next_out: target-critic outputs at (obs2, act2); z1_next / z2_next: standard-normal noise of the two
+ *           target samples.  mean_std: DEVICE float[2], the running means of the critics' std, updated in place
+ *           ((1 - tau_b) m + tau_b mean(std), or seeded with mean(std) where bit i of mean_std_unset is set) before the
+ *           loss uses them.  Writes d loss / d (mean, raw std) of both critics and out9 = {loss_q, mean q1, mean q2, mean std1,
+ *           mean std2, min std1, min std2, mean_std1, mean_std2}.
+ * policy_loss: dsact.py:315-329 on the critic outputs at (obs, new_act): mean(alpha logp - min(q1, q2)).  d_q1_out /
+ *           d_q2_out get -1/B on the mean of the smaller critic (half each on a tie), zero elsewhere; out5 as
+ *           gops_b200_dsac_policy_loss.
+ * sample_backward: gops_b200_dsac_sample_backward with d loss / d act = d_act_1 + d_act_2 (the two critics' input
+ *           gradients, same ldda). */
+int gops_b200_dsact_q_loss(const float* q1_out, const float* q2_out, const float* q1_next_out, const float* q2_next_out,
+                           const float* z1_next, const float* z2_next, const float* logp_next, const float* rew,
+                           const float* done, int64_t batch, float gamma, float alpha, double tau_b, float* mean_std,
+                           int32_t mean_std_unset, float* d_q1_out, float* d_q2_out, float* out9, void* stream);
+int gops_b200_dsact_policy_loss(const float* q1_out, const float* q2_out, const float* logp_new, int64_t batch,
+                                float alpha, float target_entropy, float* d_q1_out, float* d_q2_out, float* out5,
+                                const float* stats, void* stream);
+int gops_b200_dsact_sample_backward(const float* logits, const float* eps, int64_t batch, int32_t act_dim,
+                                    float min_log_std, float max_log_std, const float* act_half, const float* d_act_1,
+                                    const float* d_act_2, int32_t ldda, int32_t act_col0, float logp_coeff,
+                                    float* d_logits, void* stream);
 
 /* ---- data-parallel gradient exchange over NVLink peer memory, fused with Adam (peer.cu) ---------------------------
  * Replaces the gradient hand-over between replicas of the reference's synchronous trainer
