@@ -228,7 +228,7 @@ struct gops_b200_plan {
   NetL pol_tcf, val_tcf;
   int w_floats_tcf = 0;
   float *blob_pol_tcf = nullptr, *blob_val_tcf = nullptr, *blob_vtg_tcf = nullptr;
-  bool tc_attr_set[4] = {}, tc2_attr_set[4] = {};
+  bool tc2_attr_set[4] = {};
   float* osc = nullptr;   // obs scale | shift, 2 * obs_dim floats
   bool attr_set[4][4] = {};   // [alg][cfg]
   bool timing = false;
@@ -293,10 +293,11 @@ bool rollout_use_tc(const gops_b200_plan* pl, long long batch) {
   if (e && !strcmp(e, "tc")) path = GOPS_PATH_TC;
   if (path == GOPS_PATH_MMA) return false;
   if (path == GOPS_PATH_TC) return true;
-  // the wgmma kernel schedules single 128-sample sub-tiles; below ~2^14 samples (fewer sub-tiles than SMs) the mma.sync
-  // kernel with its 32-sample tiles spreads the batch over more SMs and finishes first.  Measured on one H100 80GB HBM3
-  // (700 W), ms per update mma / wgmma: FHADP idpendulum H = 30  2^13 0.74 / 0.78, 2^14 1.20 / 0.78, 2^18 11.8 / 10.4;
-  // INFADP lq s4a2 PEV + PIM  2^12 0.66 / 0.69, 2^14 0.86 / 0.71.
+  // below ~2^14 samples the mma.sync kernel with its 32-sample tiles spreads the batch over more SMs and finishes
+  // first.  Measured on one H100 80GB HBM3 (700 W) with the previous wgmma kernel (128-sample sub-tiles, one group per
+  // SM), ms per update mma / wgmma: FHADP idpendulum H = 30  2^13 0.74 / 0.78, 2^14 1.20 / 0.78, 2^18 11.8 / 10.4;
+  // INFADP lq s4a2 PEV + PIM  2^12 0.66 / 0.69, 2^14 0.86 / 0.71.  The current kernel (64-sample sub-tiles, three per
+  // SM) is faster at 2^18; its crossover has not been re-measured.
   return batch >= 16384;
 }
 __global__ void pack_params_tcf_kernel(const float* __restrict__ flat, NetL L, float* __restrict__ blob) {
@@ -618,11 +619,10 @@ int launch_rollout(gops_b200_plan* pl, const gops_b200_batch* b, int alg, cudaSt
   }
   KParams& kp = pl->kp;
   if (rollout_use_tc(pl, b->batch)) {
-    const bool v1 = false;
     const int hact = (alg == ALG_FHADP || pl->pol_tcf.hact == pl->val_tcf.hact) ? pl->pol_tcf.hact : -1;
     RolloutFn fn = rollout_fn_tc2(pl->desc.model, alg, hact);
     if (!fn) return fail("wgmma rollout kernel not built for this env model");
-    const int S = 128, NT = v1 ? 512 : tc2::NT2;
+    const int S = tc2::GT, NT = tc2::NT2;
     KParams k2 = kp;
     k2.pol = pl->pol_tcf;
     k2.val = pl->val_tcf;
@@ -643,17 +643,17 @@ int launch_rollout(gops_b200_plan* pl, const gops_b200_batch* b, int alg, cudaSt
     k2.dw_floats = round4(upd.nacc);
     const size_t smem = tc2::smem_bytes(k2.w_floats);
     if (smem > (size_t)pl->max_smem) return fail("wgmma rollout kernel does not fit in shared memory");
-    bool& attr = v1 ? pl->tc_attr_set[alg] : pl->tc2_attr_set[alg];
+    bool& attr = pl->tc2_attr_set[alg];
     if (!attr) {
       CUDA_OK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, pl->max_smem));
       attr = true;
     }
-    const long long slots = pl->sm_count;          // one CTA per SM (shared memory)
+    // one CTA per SM (shared memory); a batch of fewer sub-tiles than SMs gets one CTA per sub-tile, so that it spreads
+    // over the SMs (the kernel leaves the other warpgroups of such a CTA idle)
     const long long subtiles = (b->batch + S - 1) / S;
-    const int rows = v1 ? 1 : tc2::NG;             // gradient partial rows (= independent groups) per CTA
-    const long long want = (subtiles + rows - 1) / rows;
-    const int grid = (int)(want < slots ? want : slots);
-    if (ensure_scratch(pl, grid, v1 ? NT : tc2::NG * tc2::GT, k2.horizon, rows)) return 1;   // tape columns per CTA
+    const int grid = (int)(subtiles < pl->sm_count ? subtiles : pl->sm_count);
+    const int rows = tc2::WGS;                     // gradient partial rows (= independent warpgroups) per CTA
+    if (ensure_scratch(pl, grid, tc2::WGS * tc2::GT, k2.horizon, rows)) return 1;   // tape columns per CTA
     k2.tape = pl->tape;
     k2.ext_ref = pl->ext_ref;
     k2.xbuf = pl->xbuf;

@@ -1,5 +1,5 @@
 // BF16x3 operand primitives of the warpgroup tensor-core kernels (rollout_tc2.cuh, dense_tc.cuh): operand descriptors
-// of the canonical plane layout, the fp32 -> three-plane split and the transposing warp reduction.
+// of the canonical plane layout and the fp32 -> three-plane split.
 //
 // Arithmetic: BF16x3.  x = b0 + b1 + b2 (three bf16 planes, residual <= 2^-27 |x|), a product keeps the six terms of
 // order <= 2 (b0b0, b0b1, b1b0, b1b1, b0b2, b2b0; neglected <= 2^-26), FP32 accumulation: at least as accurate as the
@@ -19,22 +19,22 @@ namespace gops {
 
 namespace tcf {
 constexpr int K1 = 16;                           // layer-1 K extent (inputs padded to 16)
-constexpr int HPLANE = 8 * 128 * 16;             // bytes of one hidden-activation plane ([8 chunks][128 rows][16 B])
-constexpr int XPLANE = 2 * 128 * 16;             // bytes of one observation plane
+constexpr int HPLANE = 8 * 64 * 16;              // bytes of one hidden-activation plane ([8 chunks][64 rows][16 B])
+constexpr int XPLANE = 2 * 64 * 16;              // bytes of one observation plane
 constexpr int W2PLANE = 8 * 64 * 16, W1PLANE = 2 * 64 * 16;
 constexpr int ONES_B = 2 * 16 * 16;              // bytes: [2 mn-groups][16 rows][16 B]
 
 struct Op {            // one operand: smem address of plane 0, plane stride, descriptor strides, advance per K = 16 step
   uint32_t base, pstride, lbo, sbo, kadv;
 };
-__device__ __forceinline__ Op k_act(const unsigned char* b, int plane_bytes) {     // activations K-major, 128 rows
-  return Op{smem_u32(b), (uint32_t)plane_bytes, 2048u, 128u, 4096u};
+__device__ __forceinline__ Op k_act(const unsigned char* b, int plane_bytes) {     // activations K-major, 64 rows
+  return Op{smem_u32(b), (uint32_t)plane_bytes, 1024u, 128u, 2048u};
 }
 __device__ __forceinline__ Op k_w(const unsigned char* b, int plane_bytes) {       // weights K-major, 64 rows
   return Op{smem_u32(b), (uint32_t)plane_bytes, 1024u, 128u, 2048u};
 }
-__device__ __forceinline__ Op mn_act(const unsigned char* b, int plane_bytes) {    // activations transposed: K = samples
-  return Op{smem_u32(b), (uint32_t)plane_bytes, 128u, 2048u, 256u};
+__device__ __forceinline__ Op mn_act(const unsigned char* b, int plane_bytes) {    // activations transposed: K = 64 samples
+  return Op{smem_u32(b), (uint32_t)plane_bytes, 128u, 1024u, 256u};
 }
 __device__ __forceinline__ Op mn_w(const unsigned char* b, int plane_bytes) {      // weights transposed: K = output rows
   return Op{smem_u32(b), (uint32_t)plane_bytes, 128u, 1024u, 256u};
@@ -61,56 +61,6 @@ __device__ __forceinline__ void split3(f32x2::u64 X, uint32_t& p0, uint32_t& p1,
 }
 __device__ __forceinline__ void split3(float x0, float x1, uint32_t& p0, uint32_t& p1, uint32_t& p2) {
   split3(f32x2::pk(x0, x1), p0, p1, p2);
-}
-
-// 16 values of thread (q, c) -> its two 16-byte chunks (kc = 2c, 2c+1) of row r in the three planes of `buf`
-__device__ __forceinline__ void store16(unsigned char* buf, int plane_bytes, int c, int r, const float* v) {
-  uint32_t w[3][8];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) split3(v[2 * i], v[2 * i + 1], w[0][i], w[1][i], w[2][i]);
-#pragma unroll
-  for (int p = 0; p < 3; ++p) {
-    uint4* dst = reinterpret_cast<uint4*>(buf + p * plane_bytes + ((2 * c) * 128 + r) * 16);
-    dst[0] = make_uint4(w[p][0], w[p][1], w[p][2], w[p][3]);
-    dst[128] = make_uint4(w[p][4], w[p][5], w[p][6], w[p][7]);      // next chunk: + 128 rows * 16 B
-  }
-}
-
-__device__ __forceinline__ int col16(int lane) {
-  return ((lane & 16) ? 8 : 0) + ((lane & 8) ? 4 : 0) + ((lane & 4) ? 2 : 0) + ((lane & 2) ? 1 : 0);
-}
-// sum over the warp's 32 lanes of 16 per-lane values: on return v[0] of lane l holds column col16(l)
-__device__ __forceinline__ void warp_reduce16(float* v, int lane) {
-  {
-    const bool up = lane & 16;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float send = up ? v[i] : v[i + 8], keep = up ? v[i + 8] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-    }
-  }
-  {
-    const bool up = lane & 8;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float send = up ? v[i] : v[i + 4], keep = up ? v[i + 4] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-    }
-  }
-  {
-    const bool up = lane & 4;
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const float send = up ? v[i] : v[i + 2], keep = up ? v[i + 2] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-    }
-  }
-  {
-    const bool up = lane & 2;
-    const float send = up ? v[0] : v[1], keep = up ? v[1] : v[0];
-    v[0] = keep + __shfl_xor_sync(0xffffffffu, send, 2);
-  }
-  v[0] += __shfl_xor_sync(0xffffffffu, v[0], 1);
 }
 
 }  // namespace tcf

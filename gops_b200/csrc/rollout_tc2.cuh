@@ -1,28 +1,34 @@
-// Fused wgmma rollout kernel (64-wide nets, <= 16 inputs, state == obs models): one 256-thread group per CTA owning one
-// 128-sample sub-tile at a time.
+// Fused wgmma rollout kernel (64-wide nets, <= 16 inputs, state == obs models): every warpgroup of the CTA owns one
+// 64-sample sub-tile at a time and walks it through the whole horizon on its own.
 //
-//   row = sample.  Each sample row is served by a thread PAIR (h = 0 owner in warpgroup 0, h = 1 helper in warpgroup 1,
-//   both with r = thread index in the warpgroup).  The owner keeps the sample's model state and adjoint in registers
-//   for the whole horizon, runs the dynamics / adjoint and writes the observation row straight into the bf16x3 operand
-//   planes; owner and helper each read their 32 accumulator columns of the row back, apply bias / activation / output
-//   layer and multiply their deltas.  The only other exchange is the helper's half of the output dot product and the
-//   owner's output adjoint (4 KB).
+//   row = sample.  Every dense product is one warpgroup MMA (wgmma, M = 64 = the sub-tile) whose FP32 fragment stays in
+//   registers: thread t (warp w = t / 32, lane l) holds rows 16 w + l / 4 and 16 w + l / 4 + 8, columns 8 j + 2 (l % 4)
+//   + {0, 1} (wgmma.cuh).  Bias, activation, act', the split into bf16 planes, the output layer (summed over the four
+//   lanes of a quad by shuffles), delta2 = act'(pre2) * (W3^T zbar) and delta1 = (delta2 . W2) * act'(pre1) are all
+//   computed on that fragment; act'(layer 1) stays in registers from the recompute until delta1 is formed.
+//   Lanes 4q and 4q + 1 of warp w own rows 16 w + q and 16 w + q + 8: they keep the sample's model state and adjoint for
+//   the whole horizon, run the dynamics / adjoint and write the observation row into the operand planes.  z, zbar and
+//   the input gradient move within the quad by shuffles.
 //
-//   Every dense product is a warpgroup MMA (wgmma, M = 64): warpgroup h computes rows [64 h, 64 h + 64) of the 128-row
-//   layer / delta / input-gradient products and stores its register fragments into a row-major fp32 accumulator tile in
-//   shared memory, from which the row owners read.  The reductions over samples run on the tensor core as well
-//   (MN-major view of the same operand planes): warpgroup 0 forms dW2 / dW1, warpgroup 1 db2 / db1 (against a column
-//   of ones), and each adds its fragment straight into the group's FP32 global partial after every horizon step.
-//   dW3 / db3 are warp shuffles.
+//   The reductions over samples run on the tensor core as well (MN-major view of the same operand planes, K = 64):
+//   dW2 / db2 / dW1 / db1 (db against a column of ones).  Each fragment is added into the warpgroup's own FP32 global
+//   partial with red.global.add: every address of a partial has one writing thread, which adds in program order, so
+//   the gradient is bit-reproducible, and no load sits on the critical path.  dW3 / db3 are shuffle / register sums,
+//   written once at the end.
+//
+// Synchronisation: a warpgroup meets only itself (128-thread named barrier, fence.proxy.async before a wgmma reads
+// planes the threads just wrote).  FHADP has no CTA-wide barrier after the initial weight stage; INFADP swaps weight
+// blobs (policy <-> v_target <-> v) through the one staging buffer, CTA-wide, so there all warpgroups of a CTA run the
+// same number of (possibly empty) sub-tile iterations.
 //
 // Arithmetic (bars: loss 1e-4, gradient 2e-4 against the CPU oracle):
 //   layer products        x . W^T      BF16x3 x BF16x3, six terms (FP32-accurate; the loss depends on these)
 //   delta / input grad    delta . W    delta in TWO bf16 planes (2^-17 relative: the gradient bar is 2e-4), W in three
 //   weight gradients      delta^T . h  (delta_b0 + delta_b1) . (h_b0 + h_b1): four terms, FP32 accumulation
 //
-// Shared memory (~206 KB of 227): weights 31.5 KB (TMA-staged) + H1 planes 48 KB, delta planes 32 KB (delta2, then delta1
-// in the same buffer), observation planes 12 KB, exchange 4 KB, accumulator tiles: products 34 KB, act'(layer 1) 34 KB,
-// input gradient 10 KB.
+// Shared memory (~188 KB of 227 with three warpgroups): weights 31.5 KB (TMA-staged), ones 0.5 KB, and per warpgroup
+// H1 planes 24 KB, delta planes 16 KB (delta2, then delta1 in the same buffer), observation planes 2 x 6 KB (double
+// buffered by horizon step: the dW1 product of step k still reads step k's rows while step k - 1 writes its own).
 #pragma once
 #include "models.cuh"
 #include "mlp_tc_full.cuh"
@@ -30,23 +36,17 @@
 namespace gops {
 namespace tc2 {
 
-constexpr int GT = 128;                 // rows (= samples) per sub-tile = two wgmma M = 64 halves
-constexpr int GTH = 256;                // threads per group: owner warpgroup (h = 0) + helper warpgroup (h = 1)
-constexpr int NG = 1;                   // groups per CTA
-constexpr int NT2 = GTH * NG;
-constexpr int AS = 68, XS = 20;         // row strides (floats) of the accumulator tiles (padded: conflict-free row reads)
+constexpr int WGS = 3;                  // warpgroups (= independent sub-tiles) per CTA
+constexpr int GT = 64;                  // rows (= samples) per sub-tile = wgmma M
+constexpr int NT2 = 128 * WGS;          // threads per CTA
 constexpr int HPL = tcf::HPLANE, XPL = tcf::XPLANE;
 constexpr int P_BYTES = 3 * HPL, Q_BYTES = 2 * HPL, XP_BYTES = 3 * XPL;
-constexpr int XCH_BYTES = 2 * GT * MAXA * 4;   // helper -> owner output partials | owner -> helper output adjoints
-constexpr int ACC_BYTES = GT * AS * 4, DX_BYTES = GT * XS * 4;
-constexpr int GROUP_BYTES = P_BYTES + Q_BYTES + XP_BYTES + XCH_BYTES + 2 * ACC_BYTES + DX_BYTES;
+constexpr int GROUP_BYTES = P_BYTES + Q_BYTES + 2 * XP_BYTES;
 constexpr int HDR_BYTES = 256;
 
 __host__ __device__ inline size_t smem_bytes(int w_floats) {
-  return HDR_BYTES + (size_t)w_floats * 4 + tcf::ONES_B + (size_t)NG * GROUP_BYTES;
+  return HDR_BYTES + (size_t)w_floats * 4 + tcf::ONES_B + (size_t)WGS * GROUP_BYTES;
 }
-
-__device__ __forceinline__ void group_sync(int g) { asm volatile("bar.sync %0, 256;" ::"r"(1 + g) : "memory"); }
 
 // (x0, x1) -> packed bf16x2 words of two planes (low half = x0)
 __device__ __forceinline__ void split2(f32x2::u64 X, uint32_t& p0, uint32_t& p1) {
@@ -57,30 +57,41 @@ __device__ __forceinline__ void split2(f32x2::u64 X, uint32_t& p0, uint32_t& p1)
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(p1) : "f"(r1), "f"(r0));
 }
 
-// Per-thread view of its group's resources.  g, h, wg are warp-uniform (derived from a __shfl_sync'ed warp id).
+// FP32 add into global memory whose result is not used (no load on the issuing thread's path)
+__device__ __forceinline__ void red_add(float* p, float v) {
+  asm volatile("red.global.add.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
+}
+__device__ __forceinline__ void red_add2(float* p, float v0, float v1) {   // 8-byte aligned pair
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(v0), "f"(v1) : "memory");
+}
+
+// Per-thread view of its warpgroup's resources (kept small: everything else is an offset from P / Wsm).
 struct Grp {
-  unsigned char *P, *Q, *Xp;        // H1 planes (3), delta planes (2), observation planes (3)
-  float *zp, *zb;                   // exchange: helper -> owner output partials [128][MAXA]; owner -> helper adjoints
-  float *A, *D1, *DX;               // accumulator tiles: products [128][AS], act'(layer 1) [128][AS], input gradient [128][XS]
-  const unsigned char* ones;
-  int g, h, wg, r;                  // group, half (0 owner / 1 helper), warp in group, row (= sample of the sub-tile)
-  // staged weights of the network in use
-  const unsigned char *W1, *W2;
-  const float *W3, *b1, *b2, *b3;
+  unsigned char* P;                 // this warpgroup's planes: H1 (3) | delta (2) | observation (2 buffers of 3)
+  const float* Wsm;                 // staged weight blob of the network in use (NetL offsets); `ones` precedes it
+  int g, t, c;                      // warpgroup, thread in the warpgroup, t % 4 (column pair of the fragment)
+  int row;                          // owned row of the sub-tile (lanes 4q, 4q + 1 of a quad; see own)
+  bool own;
+  __device__ __forceinline__ unsigned char* Q() const { return P + P_BYTES; }
+  __device__ __forceinline__ unsigned char* X(int k) const { return P + P_BYTES + Q_BYTES + (k & 1) * XP_BYTES; }
+  __device__ __forceinline__ const unsigned char* ones() const {
+    return reinterpret_cast<const unsigned char*>(Wsm) - tcf::ONES_B;
+  }
+  __device__ __forceinline__ const unsigned char* W1(const NetL& L) const { return reinterpret_cast<const unsigned char*>(Wsm + L.o_w1); }
+  __device__ __forceinline__ const unsigned char* W2(const NetL& L) const { return reinterpret_cast<const unsigned char*>(Wsm + L.o_w2); }
+  __device__ __forceinline__ const float* W3(const NetL& L) const { return Wsm + L.o_w3; }
+  __device__ __forceinline__ const float* b1(const NetL& L) const { return Wsm + L.o_b1; }
+  __device__ __forceinline__ const float* b2(const NetL& L) const { return Wsm + L.o_b2; }
+  __device__ __forceinline__ const float* b3(const NetL& L) const { return Wsm + L.o_b3; }
 };
 
-__device__ __forceinline__ void bind(Grp& G, const float* Wsm, const NetL& L) {
-  G.W1 = reinterpret_cast<const unsigned char*>(Wsm + L.o_w1);
-  G.W2 = reinterpret_cast<const unsigned char*>(Wsm + L.o_w2);
-  G.W3 = Wsm + L.o_w3; G.b1 = Wsm + L.o_b1; G.b2 = Wsm + L.o_b2; G.b3 = Wsm + L.o_b3;
-}
-// make this thread's shared-memory writes visible to the tensor core, then meet the group
+// make this thread's shared-memory writes visible to the tensor core, then meet the warpgroup
 __device__ __forceinline__ void publish(const Grp& G) {
   fence_proxy_async();
-  group_sync(G.g);
+  wg::wg_sync(G.g);
 }
 
-// A . B^T with the six BF16x3 terms (small ones first), KS steps of K = 16; A K-major (this warpgroup's 64 rows)
+// A . B^T with the six BF16x3 terms (small ones first), KS steps of K = 16; A K-major (the sub-tile's 64 rows)
 template <int N, int TB, int KS>
 __device__ __forceinline__ void mma6(float* d, const tcf::Op& A, const tcf::Op& B) {
   using namespace tcf;
@@ -113,7 +124,7 @@ __device__ __forceinline__ void mma_dw(float* d, const tcf::Op& A, const tcf::Op
 #pragma unroll
   for (int ks = 0; ks < KS; ++ks) wg::mma_bf16<N, 0, 1>(d, a0 + ks * ka, b0 + ks * kb, 1u);
 }
-// weight gradient over the sub-tile's 128 samples: D = (A_b0 + A_b1)^T . (B_b0 + .. + B_b{BP-1}), both MN-major
+// weight gradient over the sub-tile's 64 samples: D = (A_b0 + A_b1)^T . (B_b0 + .. + B_b{BP-1}), both MN-major
 template <int N, int BP>
 __device__ __forceinline__ void mma_wgrad(float* d, const tcf::Op& A, const tcf::Op& B) {
   using namespace tcf;
@@ -125,366 +136,322 @@ __device__ __forceinline__ void mma_wgrad(float* d, const tcf::Op& A, const tcf:
     for (int q = 1; q >= 0; --q) {
       const uint64_t a = dsc(A, q), b = dsc(B, p);
 #pragma unroll
-      for (int ks = 0; ks < 8; ++ks) { wg::mma_bf16<N, 1, 1>(d, a + ks * ka, b + ks * kb, acc); acc = 1u; }
+      for (int ks = 0; ks < GT / 16; ++ks) { wg::mma_bf16<N, 1, 1>(d, a + ks * ka, b + ks * kb, acc); acc = 1u; }
     }
 }
-// this warpgroup's fragment of a 128-row product -> rows [64 h, 64 h + 64) of a row-major tile
-template <int N>
-__device__ __forceinline__ void store_frag(const Grp& G, float* dst, int ld, const float* d) {
+__device__ __forceinline__ tcf::Op ones_op(const Grp& G) { return tcf::Op{smem_u32(G.ones()), 0u, 128u, 256u, 0u}; }
+
+// this thread's m64n64 fragment (column pairs) -> NP bf16 planes of `buf` (BF16x3 for NP = 3, two planes for NP = 2)
+template <int NP>
+__device__ __forceinline__ void frag_to_planes(unsigned char* buf, const Grp& G, const float* v) {
 #pragma unroll
-  for (int i = 0; i < N / 2; i += 2)
-    *reinterpret_cast<float2*>(dst + (64 * G.h + wg::frag_row(G.r, i)) * ld + wg::frag_col(G.r, i)) = make_float2(d[i], d[i + 1]);
-}
-// this warpgroup's fragment of a [64 output rows][N] weight gradient added into the FP32 partial (row stride ld,
-// columns < ncols)
-template <int N>
-__device__ __forceinline__ void add_frag(float* __restrict__ dst, int ld, int ncols, const float* d, int r) {
-#pragma unroll
-  for (int i = 0; i < N / 2; ++i) {
-    const int row = wg::frag_row(r, i), col = wg::frag_col(r, i);
-    if (col < ncols) dst[row * ld + col] += d[i];
+  for (int i = 0; i < 32; i += 2) {
+    const int off = (i >> 2) * (GT * 16) + wg::frag_row(G.t, i) * 16 + 4 * G.c;
+    uint32_t w0, w1, w2;
+    if constexpr (NP == 3) tcf::split3(v[i], v[i + 1], w0, w1, w2);
+    else split2(f32x2::pk(v[i], v[i + 1]), w0, w1);
+    *reinterpret_cast<uint32_t*>(buf + off) = w0;
+    *reinterpret_cast<uint32_t*>(buf + HPL + off) = w1;
+    if constexpr (NP == 3) *reinterpret_cast<uint32_t*>(buf + 2 * HPL + off) = w2;
   }
 }
-// the group's 128-row product A . B^T (A = k_act(...) planes, six terms) into the product tile; ends with the group
-// barrier: the results are visible and every wgmma operand read has retired
-template <int KS>
-__device__ __forceinline__ void layer_product(const Grp& G, const tcf::Op& Ain, const tcf::Op& B) {
-  tcf::Op A = Ain;
-  A.base += 1024u * G.h;                          // + 8 row groups of 128 B
-  float d[32];
-  wg::fence();
-  mma6<64, 0, KS>(d, A, B);
-  wg::commit();
-  wg::wait<0>();
-  store_frag<64>(G, G.A, AS, d);
-  group_sync(G.g);
-}
-__device__ __forceinline__ void read16(const float* src, float* v) {
+// a [64 output rows][N] weight-gradient fragment added into the FP32 partial (row stride ld, columns < ncols);
+// PAIRS: ld and dst even, so adjacent columns go as one 8-byte add
+template <int N, bool PAIRS>
+__device__ __forceinline__ void red_frag(float* __restrict__ dst, int ld, int ncols, const float* d, int t) {
 #pragma unroll
-  for (int q = 0; q < 4; ++q) {
-    const float4 x = reinterpret_cast<const float4*>(src)[q];
-    v[4 * q] = x.x; v[4 * q + 1] = x.y; v[4 * q + 2] = x.z; v[4 * q + 3] = x.w;
+  for (int i = 0; i < N / 2; i += 2) {
+    const int row = wg::frag_row(t, i), col = wg::frag_col(t, i);
+    if constexpr (PAIRS) {
+      red_add2(dst + row * ld + col, d[i], d[i + 1]);
+    } else {
+      if (col < ncols) red_add(dst + row * ld + col, d[i]);
+      if (col + 1 < ncols) red_add(dst + row * ld + col + 1, d[i + 1]);
+    }
+  }
+}
+// column 0 of an m64n16 fragment (a product against the ones column) -> the bias gradient
+__device__ __forceinline__ void red_bias(float* __restrict__ dst, const float* d, const Grp& G) {
+  if (G.c == 0) {
+    red_add(dst + wg::frag_row(G.t, 0), d[0]);
+    red_add(dst + wg::frag_row(G.t, 2), d[2]);
   }
 }
 
-// owner: this row's input (K1 = 16 values, zero padded) -> the three observation planes.  nch = 1: the inputs fit the
-// first 8-feature chunk (idpendulum: 6 + time), the second chunk was zeroed once at kernel start.
-__device__ __forceinline__ void write_x_row(const Grp& G, const float* x, int nch) {
+// owner: this row's input (K1 = 16 values, zero padded) -> the three observation planes of buffer `x`.  nch = 1: the
+// inputs fit the first 8-feature chunk (idpendulum: 6 + time), the second chunk was zeroed once at kernel start.
+template <int NS>
+__device__ __forceinline__ void put_x(const Grp& G, unsigned char* x, const NetL& L, const float* st, float vt) {
   using namespace tcf;
+  if (!G.own) return;
+  float v[16];
+#pragma unroll
+  for (int f = 0; f < 16; ++f) v[f] = (f < NS && f < L.obs) ? st[f < NS ? f : 0] : 0.f;
+  if (L.time_input) {
+#pragma unroll
+    for (int f = 0; f < 16; ++f)
+      if (f == L.in - 1) v[f] = vt;
+  }
+  const int nch = L.in <= 8 ? 1 : 2;
 #pragma unroll
   for (int ch = 0; ch < 2; ++ch) {
     if (ch >= nch) break;
     uint32_t w[3][4];
 #pragma unroll
-    for (int i = 0; i < 4; ++i) split3(x[8 * ch + 2 * i], x[8 * ch + 2 * i + 1], w[0][i], w[1][i], w[2][i]);
+    for (int i = 0; i < 4; ++i) split3(v[8 * ch + 2 * i], v[8 * ch + 2 * i + 1], w[0][i], w[1][i], w[2][i]);
 #pragma unroll
     for (int p = 0; p < 3; ++p)
-      *reinterpret_cast<uint4*>(G.Xp + p * XPL + (ch * 128 + G.r) * 16) = make_uint4(w[p][0], w[p][1], w[p][2], w[p][3]);
+      *reinterpret_cast<uint4*>(x + p * XPL + (ch * GT + G.row) * 16) = make_uint4(w[p][0], w[p][1], w[p][2], w[p][3]);
   }
 }
 
-// layer 1, first half: observation planes . W1^T into the product tile
-template <int NS>
-__device__ __forceinline__ void layer1_issue(Grp& G, const NetL& L, const float* st, float vt) {
-  using namespace tcf;
-  if (G.h == 0) {
-    float x[16];
-#pragma unroll
-    for (int f = 0; f < 16; ++f) x[f] = (f < NS && f < L.obs) ? st[f < NS ? f : 0] : 0.f;
-    if (L.time_input) {
-#pragma unroll
-      for (int f = 0; f < 16; ++f)
-        if (f == L.in - 1) x[f] = vt;
-    }
-    write_x_row(G, x, L.in <= 8 ? 1 : 2);
-  }
-  publish(G);
-  layer_product<1>(G, k_act(G.Xp, XPL), k_w(G.W1, W1PLANE));
-}
 // AF: hidden activation fixed at compile time (>= 0), or -1 = dispatch on the runtime id.  With the activation fixed (the
 // headline configurations use GELU) the other six epilogue variants are not compiled in.
 #define GOPS_TC2_ACT_SWITCH(AF, act, M)     \
   if constexpr ((AF) >= 0) { M(AF); }       \
   else { GOPS_ACT_SWITCH(act, M) }
 
-// layer 1, second half: + b1, activation -> this thread's columns of the H1 planes (FULL: act' into the D1 tile).
-// [lo, hi): the 16-column blocks of the row this thread converts (forward sweep: owner 0-1, helper 2-3; reverse sweep:
-// the helper takes all four while the owner runs the adjoint of the dynamics).
-template <bool FULL, int AF>
-__device__ __forceinline__ void layer1_finish(Grp& G, const NetL& L, int lo, int hi) {
+// layer 1, issue: observation planes of buffer x . W1^T -> d (asynchronous; layer1_finish waits)
+__device__ __forceinline__ void layer1_issue(const Grp& G, const NetL& L, const unsigned char* x, float* d) {
   using namespace tcf;
-#pragma unroll 1
-  for (int c16 = lo; c16 < hi; ++c16) {
-    float v[16], d[16];
-    read16(G.A + G.r * AS + 16 * c16, v);
-    const float* bias = G.b1 + 16 * c16;
-#define GOPS_TC2_A1(A)                                                      \
-  _Pragma("unroll") for (int e = 0; e < 16; e += 2) {                                         \
-    const f32x2::u64 pre = f32x2::add(f32x2::pk(v[e], v[e + 1]), f32x2::ld(bias + e));       \
-    if constexpr (FULL) act_fwd_grad_pair_t<A>(pre, v[e], v[e + 1], d[e], d[e + 1]);          \
-    else act_fwd_pair_t<A>(pre, v[e], v[e + 1]);                                              \
+  publish(G);                                     // observation rows visible
+  wg::fence();
+  mma6<64, 0, 1>(d, k_act(x, XPL), k_w(G.W1(L), W1PLANE));
+  wg::commit();
+}
+// layer 1, epilogue: + b1, activation -> H1 planes; FULL: act'(pre1) into a1p
+template <bool FULL, int AF>
+__device__ __forceinline__ void layer1_finish(const Grp& G, const NetL& L, float* d, float* a1p) {
+  wg::wait<0>();
+  wg::reg_fence<32>(d);
+#define GOPS_TC2_A1(A)                                                                             \
+  _Pragma("unroll") for (int i = 0; i < 32; i += 2) {                                              \
+    const f32x2::u64 pre = f32x2::add(f32x2::pk(d[i], d[i + 1]), f32x2::ld(G.b1(L) + wg::frag_col(G.t, i))); \
+    if constexpr (FULL) act_fwd_grad_pair_t<A>(pre, d[i], d[i + 1], a1p[i], a1p[i + 1]);           \
+    else act_fwd_pair_t<A>(pre, d[i], d[i + 1]);                                                   \
   }
-    GOPS_TC2_ACT_SWITCH(AF, L.hact, GOPS_TC2_A1)
+  GOPS_TC2_ACT_SWITCH(AF, L.hact, GOPS_TC2_A1)
 #undef GOPS_TC2_A1
-    store16(G.P, HPL, c16, G.r, v);
-    if constexpr (FULL) {
+  frag_to_planes<3>(G.P, G, d);
+}
+
+// layer 2 product H1 . W2^T -> d (waited)
+__device__ __forceinline__ void layer2_product(const Grp& G, const NetL& L, float* d) {
+  using namespace tcf;
+  publish(G);                                     // H1 planes visible
+  wg::fence();
+  mma6<64, 0, 4>(d, k_act(G.P, HPL), k_w(G.W2(L), W2PLANE));
+  wg::commit();
+  wg::wait<0>();
+  wg::reg_fence<32>(d);
+}
+// output layer: S[q][a] = this thread's (even, odd) column sums of W3[a] . h for fragment row q; reduced over the four
+// lanes of the quad, the owner of each row takes z[a] = b3[a] + W3[a] . h
+__device__ __forceinline__ void output_sum(const Grp& G, const NetL& L, f32x2::u64 (*S)[MAXA], float* z) {
 #pragma unroll
-      for (int q = 0; q < 4; ++q)
-        reinterpret_cast<float4*>(G.D1 + G.r * AS + 16 * c16)[q] = make_float4(d[4 * q], d[4 * q + 1], d[4 * q + 2], d[4 * q + 3]);
+  for (int a = 0; a < MAXA; ++a) {
+    z[a] = 0.f;
+    if (a < L.out) {
+      float s[2];
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        float s0, s1;
+        f32x2::upk(S[q][a], s0, s1);
+        s[q] = s0 + s1;
+        s[q] += __shfl_xor_sync(0xffffffffu, s[q], 1);
+        s[q] += __shfl_xor_sync(0xffffffffu, s[q], 2);
+      }
+      z[a] = G.b3(L)[a] + (G.c == 0 ? s[0] : s[1]);
     }
   }
+}
+__device__ __forceinline__ void output_layer(const Grp& G, const NetL& L, const float* h, float* z) {
+  f32x2::u64 S[2][MAXA];
+#pragma unroll
+  for (int a = 0; a < MAXA; ++a) S[0][a] = S[1][a] = f32x2::rep(0.f);
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) {
+    const int col = wg::frag_col(G.t, i), q = (i >> 1) & 1;
+#pragma unroll
+    for (int a = 0; a < MAXA; ++a)
+      if (a < L.out) S[q][a] = f32x2::fma(f32x2::ld(G.W3(L) + a * 64 + col), f32x2::pk(h[i], h[i + 1]), S[q][a]);
+  }
+  output_sum(G, L, S, z);
 }
 
 // layer 2 + output layer, forward only: the owner gets z[a] = b3[a] + W3[a] . act(H1 . W2^T + b2)
 template <int AF>
-__device__ __forceinline__ void layer2_out(Grp& G, const NetL& L, float* z) {
-  using namespace tcf;
-  publish(G);
-  layer_product<4>(G, k_act(G.P, HPL), k_w(G.W2, W2PLANE));
-  float zp[MAXA];
-#pragma unroll
-  for (int a = 0; a < MAXA; ++a) zp[a] = 0.f;
-#pragma unroll 1
-  for (int cb = 0; cb < 2; ++cb) {
-    const int c16 = 2 * G.h + cb;
-    float v[16];
-    read16(G.A + G.r * AS + 16 * c16, v);
-    const float* bias = G.b2 + 16 * c16;
-#define GOPS_TC2_A2(A)                               \
-  _Pragma("unroll") for (int e = 0; e < 16; e += 2)  \
-      act_fwd_pair_t<A>(f32x2::add(f32x2::pk(v[e], v[e + 1]), f32x2::ld(bias + e)), v[e], v[e + 1]);
-    GOPS_TC2_ACT_SWITCH(AF, L.hact, GOPS_TC2_A2)
+__device__ __forceinline__ void layer2_out(const Grp& G, const NetL& L, float* z) {
+  float d[32];
+  layer2_product(G, L, d);
+#define GOPS_TC2_A2(A)                                \
+  _Pragma("unroll") for (int i = 0; i < 32; i += 2)   \
+      act_fwd_pair_t<A>(f32x2::add(f32x2::pk(d[i], d[i + 1]), f32x2::ld(G.b2(L) + wg::frag_col(G.t, i))), d[i], d[i + 1]);
+  GOPS_TC2_ACT_SWITCH(AF, L.hact, GOPS_TC2_A2)
 #undef GOPS_TC2_A2
-#pragma unroll
-    for (int a = 0; a < MAXA; ++a)
-      if (a < L.out) {
-        const float* w = G.W3 + a * 64 + 16 * c16;
-        f32x2::u64 S = f32x2::rep(0.f);           // (even, odd) column partial sums
-#pragma unroll
-        for (int e = 0; e < 16; e += 2) S = f32x2::fma(f32x2::ld(w + e), f32x2::pk(v[e], v[e + 1]), S);
-        float s0, s1;
-        f32x2::upk(S, s0, s1);
-        zp[a] += s0 + s1;
-      }
-  }
-  if (G.h == 1) {
-#pragma unroll
-    for (int a = 0; a < MAXA; ++a)
-      if (a < L.out) G.zp[G.r * MAXA + a] = zp[a];
-  }
-  group_sync(G.g);
-  if (G.h == 0) {
-#pragma unroll
-    for (int a = 0; a < MAXA; ++a) z[a] = a < L.out ? G.b3[a] + (zp[a] + G.zp[G.r * MAXA + a]) : 0.f;
-  }
+  output_layer(G, L, d, z);
 }
 
-// Per-thread accumulators of the output-layer gradients: after the transposing warp reduction lane l holds the warp's
-// column sum of column 32 h + 16 q + col16(l) in slot q; they are combined across warps once, at the end of the kernel.
+// Per-thread accumulators of the output-layer gradients: lane l of warp w holds dW3[a] of columns 8 (l / 4) + 2 (l % 4)
+// + {0, 1}, summed over the warp's 16 rows; the owners hold their rows' db3.  Combined across the warps once, at the end
+// of the kernel.
 struct Acc3 {
-  float w0[MAXA], w1[MAXA];
+  float w[MAXA][2];
   float b[MAXA];
 };
 
-// layer 2 recompute fused with the start of the backward pass: z for the owner (WANT_Z), dW3 / db3 partial sums, and
-// delta2 = (W3^T zbar) * act'(pre2) -> this thread's 32 columns of the two delta planes.
-// zbar: the owner's output adjoint of its row (the helper receives it through shared memory).
-template <bool WANT_DW, bool WANT_Z, int AF>
-__device__ __forceinline__ void layer2_back(Grp& G, const NetL& L, const float* zbar, float* z, Acc3& acc3) {
-  using namespace tcf;
-  if (G.h == 0) {
+// layer 2 epilogue of the backward pass, one column pair of both fragment rows at a time: h = act(pre2), then
+// delta2 = act'(pre2) * (W3^T zbar) straight into the two delta planes, WANT_DW: the dW3 sums (over the warp's rows by
+// an xor butterfly over the quads), WANT_Z: the output-layer partial sums S (output_layer).  zr: zbar of the two rows.
+template <int A, bool WANT_DW, bool WANT_Z>
+__device__ __forceinline__ void delta2_epilogue(const Grp& G, const NetL& L, float* d, const float (*zr)[MAXA], Acc3& acc3,
+                                                f32x2::u64 (*S)[MAXA]) {
+  const int q4 = (G.t & 31) >> 2;
 #pragma unroll
-    for (int a = 0; a < MAXA; ++a)
-      if (a < L.out) G.zb[G.r * MAXA + a] = zbar[a];
-  }
-  publish(G);
-  layer_product<4>(G, k_act(G.P, HPL), k_w(G.W2, W2PLANE));
-  float zb[MAXA];
+  for (int j = 0; j < 8; ++j) {
+    const int col = 8 * j + 2 * G.c;
+    float h[2][2];
 #pragma unroll
-  for (int a = 0; a < MAXA; ++a) zb[a] = a < L.out ? G.zb[G.r * MAXA + a] : 0.f;
-  const int lane = G.r & 31;
-  float zp[MAXA];
-#pragma unroll
-  for (int a = 0; a < MAXA; ++a) zp[a] = 0.f;
-#pragma unroll 1
-  for (int cb = 0; cb < 2; ++cb) {
-    const int c16 = 2 * G.h + cb;
-    float v[16], d[16];
-    read16(G.A + G.r * AS + 16 * c16, v);
-    const float* bias = G.b2 + 16 * c16;
-#define GOPS_TC2_A3(A)                               \
-  _Pragma("unroll") for (int e = 0; e < 16; e += 2)  \
-      act_fwd_grad_pair_t<A>(f32x2::add(f32x2::pk(v[e], v[e + 1]), f32x2::ld(bias + e)), v[e], v[e + 1], d[e], d[e + 1]);
-    GOPS_TC2_ACT_SWITCH(AF, L.hact, GOPS_TC2_A3)
-#undef GOPS_TC2_A3
-    const float* w3 = G.W3 + 16 * c16;
-    if constexpr (WANT_Z) {
-#pragma unroll
-      for (int a = 0; a < MAXA; ++a)
-        if (a < L.out) {
-          f32x2::u64 S = f32x2::rep(0.f);
-#pragma unroll
-          for (int e = 0; e < 16; e += 2) S = f32x2::fma(f32x2::ld(w3 + a * 64 + e), f32x2::pk(v[e], v[e + 1]), S);
-          float s0, s1;
-          f32x2::upk(S, s0, s1);
-          zp[a] += s0 + s1;
-        }
-    }
-    if constexpr (WANT_DW) {
-#pragma unroll
-      for (int a = 0; a < MAXA; ++a)
-        if (a < L.out) {
-          float t[16];
-#pragma unroll
-          for (int e = 0; e < 16; e += 2) f32x2::upk(f32x2::mul(f32x2::rep(zb[a]), f32x2::pk(v[e], v[e + 1])), t[e], t[e + 1]);
-          warp_reduce16(t, lane);
-          acc3.w0[a] += cb == 0 ? t[0] : 0.f;
-          acc3.w1[a] += cb == 0 ? 0.f : t[0];
-        }
-    }
-    f32x2::u64 D2[8];                              // delta2 pairs = act'(pre2) * (W3^T zbar)
-#pragma unroll
-    for (int e = 0; e < 16; e += 2) {
+    for (int q = 0; q < 2; ++q) {
+      const int i = 4 * j + 2 * q;
+      float g0, g1;
+      act_fwd_grad_pair_t<A>(f32x2::add(f32x2::pk(d[i], d[i + 1]), f32x2::ld(G.b2(L) + col)), h[q][0], h[q][1], g0, g1);
       f32x2::u64 gs = f32x2::rep(0.f);
 #pragma unroll
       for (int a = 0; a < MAXA; ++a)
-        if (a < L.out) gs = f32x2::fma(f32x2::ld(w3 + a * 64 + e), f32x2::rep(zb[a]), gs);
-      D2[e / 2] = f32x2::mul(f32x2::pk(d[e], d[e + 1]), gs);
-    }
-    // two delta planes: chunks 2 c16, 2 c16 + 1 of row r
+        if (a < L.out) gs = f32x2::fma(f32x2::ld(G.W3(L) + a * 64 + col), f32x2::rep(zr[q][a]), gs);
+      uint32_t w0, w1;
+      split2(f32x2::mul(f32x2::pk(g0, g1), gs), w0, w1);
+      const int off = j * (GT * 16) + wg::frag_row(G.t, i) * 16 + 4 * G.c;
+      *reinterpret_cast<uint32_t*>(G.Q() + off) = w0;
+      *reinterpret_cast<uint32_t*>(G.Q() + HPL + off) = w1;
+      if constexpr (WANT_Z) {
 #pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      uint32_t w0[4], w1[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) split2(D2[4 * c + i], w0[i], w1[i]);
-      *reinterpret_cast<uint4*>(G.Q + ((2 * c16 + c) * 128 + G.r) * 16) = make_uint4(w0[0], w0[1], w0[2], w0[3]);
-      *reinterpret_cast<uint4*>(G.Q + HPL + ((2 * c16 + c) * 128 + G.r) * 16) = make_uint4(w1[0], w1[1], w1[2], w1[3]);
+        for (int a = 0; a < MAXA; ++a)
+          if (a < L.out) S[q][a] = f32x2::fma(f32x2::ld(G.W3(L) + a * 64 + col), f32x2::pk(h[q][0], h[q][1]), S[q][a]);
+      }
     }
-  }
-  if constexpr (WANT_DW) {
-    if (G.h == 0) {
+    if constexpr (WANT_DW) {
 #pragma unroll
       for (int a = 0; a < MAXA; ++a)
         if (a < L.out) {
-          float sz = zb[a];
 #pragma unroll
-          for (int o = 16; o > 0; o >>= 1) sz += __shfl_xor_sync(0xffffffffu, sz, o);
-          acc3.b[a] += sz;
+          for (int e = 0; e < 2; ++e) {
+            float v = fmaf(zr[1][a], h[1][e], zr[0][a] * h[0][e]);
+            v += __shfl_xor_sync(0xffffffffu, v, 4);
+            v += __shfl_xor_sync(0xffffffffu, v, 8);
+            v += __shfl_xor_sync(0xffffffffu, v, 16);
+            if (q4 == j) acc3.w[a][e] += v;
+          }
         }
     }
   }
-  if constexpr (WANT_Z) {
-    if (G.h == 1) {
+}
+
+// layer 2 recompute fused with the start of the backward pass: z for the owner (WANT_Z), dW3 / db3 sums, and
+// delta2 -> the two delta planes.  zbar: the owner's output adjoint of its row.
+template <bool WANT_DW, bool WANT_Z, int AF>
+__device__ __forceinline__ void layer2_back(const Grp& G, const NetL& L, const float* zbar, float* z, Acc3& acc3) {
+  float d[32];
+  layer2_product(G, L, d);
+  const int qb = (G.t & 31) & ~3;
+  float zr[2][MAXA];                              // zbar of the fragment's two rows
 #pragma unroll
-      for (int a = 0; a < MAXA; ++a)
-        if (a < L.out) G.zp[G.r * MAXA + a] = zp[a];
-    }
-    group_sync(G.g);
-    if (G.h == 0) {
+  for (int a = 0; a < MAXA; ++a) {
+    zr[0][a] = __shfl_sync(0xffffffffu, zbar[a], qb);
+    zr[1][a] = __shfl_sync(0xffffffffu, zbar[a], qb + 1);
+  }
+  f32x2::u64 S[2][MAXA];
 #pragma unroll
-      for (int a = 0; a < MAXA; ++a) z[a] = a < L.out ? G.b3[a] + (zp[a] + G.zp[G.r * MAXA + a]) : 0.f;
-    }
+  for (int a = 0; a < MAXA; ++a) S[0][a] = S[1][a] = f32x2::rep(0.f);
+#define GOPS_TC2_A3(A) delta2_epilogue<A, WANT_DW, WANT_Z>(G, L, d, zr, acc3, S);
+  GOPS_TC2_ACT_SWITCH(AF, L.hact, GOPS_TC2_A3)
+#undef GOPS_TC2_A3
+  if constexpr (WANT_Z) output_sum(G, L, S, z);
+  if constexpr (WANT_DW) {
+#pragma unroll
+    for (int a = 0; a < MAXA; ++a)
+      if (a < L.out && G.own) acc3.b[a] += zbar[a];
   }
 }
 
-// delta2 planes -> delta1 = (delta2 . W2) * act'(pre1) (same planes, once the readers of delta2 retired) -> input
-// gradient rows in the DX tile (want_dx; the owner reads them with collect_dx) and, WANT_DW, the weight gradients of both
-// layers added into the group's partial `part`: warpgroup 0 forms dW2 / dW1, warpgroup 1 db2 / db1.
-template <bool WANT_DW>
-__device__ __forceinline__ void backprop(Grp& G, const NetL& L, bool want_dx, float* __restrict__ part) {
+// delta2 planes -> delta1 = (delta2 . W2) * act'(pre1) (same planes, once the readers of delta2 retired) -> the owner's
+// input gradient dx (want_dx) and, WANT_DW, the weight gradients of both layers added into the partial `part`.
+// x: the observation planes of this step's layer 1.
+template <bool WANT_DW, int NS>
+__device__ __forceinline__ void backprop(const Grp& G, const NetL& L, bool want_dx, float* __restrict__ part,
+                                         const unsigned char* x, const float* a1p, float* dx) {
   using namespace tcf;
-  publish(G);
-  {
-    Op A = k_act(G.Q, HPL);
-    A.base += 1024u * G.h;
-    float d[32];
-    wg::fence();
-    mma_dw<64, 4>(d, A, mn_w(G.W2, W2PLANE));
-    wg::commit();
-    if constexpr (WANT_DW) {
-      const Op Ad = mn_act(G.Q, HPL);
-      if (G.h == 0) {
-        float w[32];
-        wg::fence();
-        mma_wgrad<64, 2>(w, Ad, mn_act(G.P, HPL));
-        wg::commit();
-        wg::wait<0>();
-        wg::reg_fence<32>(w);
-        add_frag<64>(part + L.g_w2, 64, 64, w, G.r);
-      } else {
-        float w[8];
-        wg::fence();
-        mma_wgrad<16, 1>(w, Ad, Op{smem_u32(G.ones), 0u, 128u, 256u, 0u});
-        wg::commit();
-        wg::wait<0>();
-        wg::reg_fence<8>(w);
-        add_frag<16>(part + L.g_b2, 1, 1, w, G.r);
-      }
-    }
-    wg::wait<0>();
-    wg::reg_fence<32>(d);
-    store_frag<64>(G, G.A, AS, d);
-  }
-  group_sync(G.g);                               // delta2 . W2 visible; every reader of delta2 / H1 has retired
+  publish(G);                                     // delta2 planes visible
+  float g1[32];
+  wg::fence();
+  mma_dw<64, 4>(g1, k_act(G.Q(), HPL), mn_w(G.W2(L), W2PLANE));
+  wg::commit();
+  wg::wait<0>();
+  wg::reg_fence<32>(g1);
   if (!WANT_DW && !want_dx) return;
-  {
-    float ra[32], rb[32];
-    read16(G.A + G.r * AS + 32 * G.h, ra);
-    read16(G.A + G.r * AS + 32 * G.h + 16, ra + 16);
-    read16(G.D1 + G.r * AS + 32 * G.h, rb);
-    read16(G.D1 + G.r * AS + 32 * G.h + 16, rb + 16);
-    uint32_t w0[16], w1[16];                     // delta1 planes of this thread's 32 columns
 #pragma unroll
-    for (int i = 0; i < 16; ++i)
-      split2(f32x2::mul(f32x2::pk(ra[2 * i], ra[2 * i + 1]), f32x2::pk(rb[2 * i], rb[2 * i + 1])), w0[i], w1[i]);
-#pragma unroll
-    for (int c = 0; c < 4; ++c) {
-      *reinterpret_cast<uint4*>(G.Q + ((4 * G.h + c) * 128 + G.r) * 16) = make_uint4(w0[4 * c], w0[4 * c + 1], w0[4 * c + 2], w0[4 * c + 3]);
-      *reinterpret_cast<uint4*>(G.Q + HPL + ((4 * G.h + c) * 128 + G.r) * 16) = make_uint4(w1[4 * c], w1[4 * c + 1], w1[4 * c + 2], w1[4 * c + 3]);
-    }
-  }
-  publish(G);
-  if (want_dx) {
-    Op A = k_act(G.Q, HPL);
-    A.base += 1024u * G.h;
-    float d[8];
+  for (int i = 0; i < 32; ++i) g1[i] *= a1p[i];   // delta1, written once the wgmma reads of delta2 have retired
+  if constexpr (WANT_DW) {
+    float w[32], wb[8];
     wg::fence();
-    mma_dw<16, 4>(d, A, mn_w(G.W1, W1PLANE));
+    mma_wgrad<64, 2>(w, mn_act(G.Q(), HPL), mn_act(G.P, HPL));
+    mma_wgrad<16, 1>(wb, mn_act(G.Q(), HPL), ones_op(G));
     wg::commit();
     wg::wait<0>();
-    wg::reg_fence<8>(d);
-    store_frag<16>(G, G.DX, XS, d);
+    wg::reg_fence<32>(w);
+    wg::reg_fence<8>(wb);
+    red_frag<64, true>(part + L.g_w2, 64, 64, w, G.t);
+    red_bias(part + L.g_b2, wb, G);
+  }
+  wg::wg_sync(G.g);                               // every wgmma read of delta2 retired
+  frag_to_planes<2>(G.Q(), G, g1);
+  publish(G);                                     // delta1 planes visible
+  float d[8], w[8], wb[8];
+  if (want_dx) {
+    wg::fence();
+    mma_dw<16, 4>(d, k_act(G.Q(), HPL), mn_w(G.W1(L), W1PLANE));
+    wg::commit();
   }
   if constexpr (WANT_DW) {
-    const Op Ad = mn_act(G.Q, HPL);
-    float w[8];
     wg::fence();
-    if (G.h == 0) mma_wgrad<16, 2>(w, Ad, mn_act(G.Xp, XPL));
-    else mma_wgrad<16, 1>(w, Ad, Op{smem_u32(G.ones), 0u, 128u, 256u, 0u});
+    mma_wgrad<16, 2>(w, mn_act(G.Q(), HPL), mn_act(x, XPL));
+    mma_wgrad<16, 1>(wb, mn_act(G.Q(), HPL), ones_op(G));
     wg::commit();
-    wg::wait<0>();
-    wg::reg_fence<8>(w);
-    if (G.h == 0) add_frag<16>(part + L.g_w1, L.in, L.in, w, G.r);
-    else add_frag<16>(part + L.g_b1, 1, 1, w, G.r);
   }
-  group_sync(G.g);                               // input gradient visible; delta1 / X planes free
-}
-
-// owner half: the input gradient of the last backprop(..., want_dx = true)
-__device__ __forceinline__ void collect_dx(const Grp& G, float* dx) {
-  float v[16];
-  read16(G.DX + G.r * XS, v);
+  wg::wait<0>();
+  if constexpr (WANT_DW) {
+    wg::reg_fence<8>(w);
+    wg::reg_fence<8>(wb);
+    red_frag<16, false>(part + L.g_w1, L.in, L.in, w, G.t);
+    red_bias(part + L.g_b1, wb, G);
+  }
+  if (want_dx) {
+    wg::reg_fence<8>(d);
+    // register i = 4 j + 2 h + e of lane 4q + c' holds row 16 w + q + 8 h, column 8 j + 2 c' + e; owner h = c
+    const int qb = (G.t & 31) & ~3;
 #pragma unroll
-  for (int f = 0; f < 16; ++f) dx[f] = v[f];
+    for (int j = 0; j < 2; ++j)
+#pragma unroll
+      for (int cc = 0; cc < 4; ++cc)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int f = 8 * j + 2 * cc + e;
+          if (f < NS) {
+            const float v0 = __shfl_sync(0xffffffffu, d[4 * j + e], qb + cc);
+            const float v1 = __shfl_sync(0xffffffffu, d[4 * j + 2 + e], qb + cc);
+            dx[f] = G.c == 0 ? v0 : v1;
+          }
+        }
+  }
 }
 
 }  // namespace tc2
 
 // ---------------------------------------------------------------------------------------------------------------
-// The kernel.  grid = min(#SM, #sub-tiles) CTAs of 256 threads, one CTA per SM (shared memory).
-// Slot s = NG * blockIdx.x + group owns the contiguous sub-tile range [NSUB s / slots, NSUB (s + 1) / slots).
-// INFADP swaps weight blobs (policy <-> v_target <-> v) through the one staging buffer: those swap points are CTA-wide
-// barriers, so with NG > 1 all groups run the same number of (possibly empty) sub-tile iterations.
+// The kernel.  grid = min(#SM, #sub-tiles) CTAs of WGS warpgroups, one CTA per SM (shared memory).
+// Slot s = WGS * blockIdx.x + warpgroup owns the contiguous sub-tile range [NSUB s / slots, NSUB (s + 1) / slots), its
+// tape columns and its row of the gradient partials.
 // ---------------------------------------------------------------------------------------------------------------
 template <class M, int ALG, int AF = -1>
 __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_constant__ KParams p) {
@@ -494,27 +461,21 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
   extern __shared__ __align__(16) float smem[];
   unsigned char* sm = reinterpret_cast<unsigned char*>(smem);
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm);           // [0] weights landed
-  float* Wsm = reinterpret_cast<float*>(sm + HDR_BYTES);
-  unsigned char* ones = sm + HDR_BYTES + (size_t)p.w_floats * 4;
-  unsigned char* gbase = ones + tcf::ONES_B;
+  unsigned char* ones = sm + HDR_BYTES;
+  float* Wsm = reinterpret_cast<float*>(ones + tcf::ONES_B);
+  unsigned char* gbase = reinterpret_cast<unsigned char*>(Wsm + p.w_floats);
 
   const int tid = threadIdx.x;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);      // warp-uniform by construction
   Grp G;
-  G.g = warp >> 3;
-  G.wg = warp & 7;
-  G.h = G.wg >> 2;
-  G.r = 32 * (G.wg & 3) + (tid & 31);
+  G.g = warp >> 2;
+  G.t = tid & 127;
+  G.c = tid & 3;
+  G.row = wg::frag_row(G.t, 2 * (G.c & 1));                   // lanes 4q, 4q + 1: rows 16 w + q, 16 w + q + 8
+  G.own = G.c < 2;
   G.P = gbase + G.g * GROUP_BYTES;
-  G.Q = G.P + P_BYTES;
-  G.Xp = G.Q + Q_BYTES;
-  G.zp = reinterpret_cast<float*>(G.Xp + XP_BYTES);
-  G.zb = G.zp + GT * MAXA;
-  G.A = reinterpret_cast<float*>(G.Xp + XP_BYTES + XCH_BYTES);
-  G.D1 = G.A + GT * AS;
-  G.DX = G.D1 + GT * AS;
-  G.ones = ones;
-  const bool own = G.h == 0;
+  G.Wsm = Wsm;
+  const bool own = G.own;
 
   if (tid == 0) {
     mbar_init(bars, 1);
@@ -525,7 +486,7 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
     o16[tid] = (tid < 128 && (tid & 7) == 0) ? (uint16_t)0x3f80 : (uint16_t)0;
   }
   uint32_t wphase = 0;
-  auto stage = [&](const float* gsrc, int floats) {      // CTA-wide: both groups call it at the same program points
+  auto stage = [&](const float* gsrc, int floats) {      // CTA-wide: every warpgroup calls it at the same program points
     __syncthreads();
     if (tid == 0) {
       fence_proxy_async();
@@ -544,37 +505,40 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
   const NetL& V = p.val;
   const int H = p.horizon, obs_dim = P.obs, TCH = p.tape_ch;
   const long long B = p.batch;
-  const int slot = blockIdx.x * NG + G.g, slots = gridDim.x * NG;
+  const int slot = blockIdx.x * WGS + G.g, slots = gridDim.x * WGS;
+  // zeroed before the first red.global.add into it: stage() below is a CTA barrier
   float* part = p.partial + (size_t)slot * p.part_stride;
-  for (int i = G.h * GT + G.r; i < p.part_stride; i += GTH) part[i] = 0.f;
+  for (int i = G.t; i < p.part_stride; i += 128) part[i] = 0.f;
   float* tape = p.tape + (size_t)slot * (size_t)H * TCH * GT;
   Acc3 acc3;
 #pragma unroll
-  for (int a = 0; a < MAXA; ++a) acc3.w0[a] = acc3.w1[a] = acc3.b[a] = 0.f;
+  for (int a = 0; a < MAXA; ++a) acc3.w[a][0] = acc3.w[a][1] = acc3.b[a] = 0.f;
   float loss_acc = 0.f, vmean_acc = 0.f, done_acc = 0.f;
 
-  for (int i = G.h * GT + G.r; i < XP_BYTES / 16; i += GTH) reinterpret_cast<uint4*>(G.Xp)[i] = make_uint4(0u, 0u, 0u, 0u);
+  for (int i = G.t; i < 2 * XP_BYTES / 16; i += 128) reinterpret_cast<uint4*>(G.X(0))[i] = make_uint4(0u, 0u, 0u, 0u);
   stage(p.blob_pol, P.blob);      // (its leading CTA barrier also publishes the zeroed planes)
-  bind(G, Wsm, P);
 
   const long long nsub = (B + GT - 1) / GT;
   const long long s0 = nsub * slot / slots, s1 = nsub * (slot + 1) / slots;
-  // INFADP: equal iteration counts for both groups of the CTA (stage() is a CTA-wide barrier)
+  // INFADP: equal iteration counts for all warpgroups of the CTA (stage() is a CTA-wide barrier)
   long long iters = s1 - s0;
-  if (NG > 1 && (alg == ALG_PIM || alg == ALG_PEV)) {
-    const long long o0 = nsub * (slot ^ 1) / slots, o1 = nsub * ((slot ^ 1) + 1) / slots;
-    iters = (o1 - o0) > iters ? (o1 - o0) : iters;
+  if (WGS > 1 && (alg == ALG_PIM || alg == ALG_PEV)) {
+    for (int o = 0; o < WGS; ++o) {
+      const long long os = (long long)blockIdx.x * WGS + o;
+      const long long n = nsub * (os + 1) / slots - nsub * os / slots;
+      iters = n > iters ? n : iters;
+    }
   }
 
   for (long long it = 0; it < iters; ++it) {
     const long long sub = s0 + it;
     const bool have = sub < s1;                   // false: idle iteration that only takes part in the blob swaps
-    const long long gs = sub * GT + G.r;
-    const bool valid = have && gs < B;
+    const long long gs = sub * GT + G.row;
+    const bool valid = own && have && gs < B;
     float st[NS];
 #pragma unroll
-    for (int f = 0; f < NS; ++f) st[f] = (own && valid && f < obs_dim) ? p.obs[gs * obs_dim + f] : 0.f;
-    bool dn = (own && valid) ? (p.done[gs] != 0.f) : true;
+    for (int f = 0; f < NS; ++f) st[f] = (valid && f < obs_dim) ? p.obs[gs * obs_dim + f] : 0.f;
+    bool dn = valid ? (p.done[gs] != 0.f) : true;
     float vacc = 0.f;
 
     // ================================ forward sweep ================================
@@ -583,20 +547,21 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
         if (own) {
           if (alg == ALG_FHADP || alg == ALG_PIM) {
 #pragma unroll
-            for (int f = 0; f < NS; ++f) tape[(k * TCH + f) * GT + G.r] = st[f];
-            tape[(k * TCH + NS) * GT + G.r] = dn ? 1.f : 0.f;
+            for (int f = 0; f < NS; ++f) tape[(k * TCH + f) * GT + G.row] = st[f];
+            tape[(k * TCH + NS) * GT + G.row] = dn ? 1.f : 0.f;
           }
         }
-        float z[MAXA];
-        layer1_issue<NS>(G, P, st, (float)(k + 1));
-        layer1_finish<false, AF>(G, P, 2 * G.h, 2 * G.h + 2);
+        float z[MAXA], d1[32];
+        put_x<NS>(G, G.X(k), P, st, (float)(k + 1));
+        layer1_issue(G, P, G.X(k), d1);
+        layer1_finish<false, AF>(G, P, d1, nullptr);
         layer2_out<AF>(G, P, z);
         if (own) {
           float a[MAXA], g[MAXA], apol[MAXA];
           if (alg == ALG_FHADP || alg == ALG_PIM) {
 #pragma unroll
             for (int j = 0; j < MAXA; ++j)
-              if (j < P.out) tape[(k * TCH + NS + 1 + j) * GT + G.r] = z[j];
+              if (j < P.out) tape[(k * TCH + NS + 1 + j) * GT + G.row] = z[j];
           }
           process_action(p, P.out, z, a, g, apol);
           const bool active = valid && (p.mask_at_done ? !dn : true);
@@ -636,7 +601,7 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           }
         }
       }
-      if (own && valid && dn) done_acc += 1.f;
+      if (valid && dn) done_acc += 1.f;
     }
     if (alg == ALG_TRACE) continue;
 
@@ -646,28 +611,27 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
     for (int f = 0; f < NS; ++f) lam[f] = 0.f;
     if (alg != ALG_FHADP) {
       stage(p.blob_vtg, V.blob);
-      bind(G, Wsm, V);
       if (have) {
         const float gn = p.gpow[H];
-        const bool term = own && valid && !dn;
-        float zv[MAXA], zb[MAXA], dx[16];
+        const bool term = valid && !dn;
+        float zv[MAXA], zb[MAXA], d1[32], a1p[32];
 #pragma unroll
         for (int j = 0; j < MAXA; ++j) zb[j] = zv[j] = 0.f;
+        put_x<NS>(G, G.X(0), V, st, 0.f);
+        layer1_issue(G, V, G.X(0), d1);
         if (alg == ALG_PIM) {
+          float dx[NS];
           zb[0] = term ? -gn * p.inv_B : 0.f;
-          layer1_issue<NS>(G, V, st, 0.f);
-          layer1_finish<true, AF>(G, V, 2 * G.h, 2 * G.h + 2);
+          layer1_finish<true, AF>(G, V, d1, a1p);
           layer2_back<false, true, AF>(G, V, zb, zv, acc3);
-          backprop<false>(G, V, true, part);
-          collect_dx(G, dx);
+          backprop<false, NS>(G, V, true, part, G.X(0), a1p, dx);
           if (term) {
 #pragma unroll
             for (int f = 0; f < NS; ++f)
               if (f < obs_dim) lam[f] = dx[f];
           }
         } else {
-          layer1_issue<NS>(G, V, st, 0.f);
-          layer1_finish<false, AF>(G, V, 2 * G.h, 2 * G.h + 2);
+          layer1_finish<false, AF>(G, V, d1, nullptr);
           layer2_out<AF>(G, V, zv);
         }
         if (term) vacc += gn * zv[0];
@@ -677,36 +641,34 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
     if (alg == ALG_PEV) {
       // loss_v = mean((v(o_0) - backup)^2), gradient w.r.t. the value net only
       stage(p.blob_val, V.blob);
-      bind(G, Wsm, V);
       if (have) {
         float o0[NS];
 #pragma unroll
-        for (int f = 0; f < NS; ++f) o0[f] = (own && valid && f < obs_dim) ? p.obs[gs * obs_dim + f] : 0.f;
-        float zv[MAXA], zb[MAXA];
+        for (int f = 0; f < NS; ++f) o0[f] = (valid && f < obs_dim) ? p.obs[gs * obs_dim + f] : 0.f;
+        float zv[MAXA], zb[MAXA], d1[32], a1p[32];
 #pragma unroll
         for (int j = 0; j < MAXA; ++j) zb[j] = zv[j] = 0.f;
         // the output adjoint needs v(o_0) first: forward to the output, then recompute layer 2 fused with the backward
-        layer1_issue<NS>(G, V, o0, 0.f);
-        layer1_finish<true, AF>(G, V, 2 * G.h, 2 * G.h + 2);
+        put_x<NS>(G, G.X(0), V, o0, 0.f);
+        layer1_issue(G, V, G.X(0), d1);
+        layer1_finish<true, AF>(G, V, d1, a1p);
         layer2_out<AF>(G, V, zv);
-        if (own && valid) {
+        if (valid) {
           const float diff = zv[0] - vacc;
           loss_acc += diff * diff * p.inv_B;
           vmean_acc += zv[0] * p.inv_B;
           zb[0] = 2.f * diff * p.inv_B;
         }
         layer2_back<true, false, AF>(G, V, zb, nullptr, acc3);
-        backprop<true>(G, V, false, part);
+        backprop<true, NS>(G, V, false, part, G.X(0), a1p, nullptr);
       }
       stage(p.blob_pol, P.blob);
-      bind(G, Wsm, P);
       continue;
     }
 
-    if (own && valid) loss_acc += -vacc * p.inv_B;
+    if (valid) loss_acc += -vacc * p.inv_B;
     if (alg == ALG_PIM) {
       stage(p.blob_pol, P.blob);
-      bind(G, Wsm, P);
     }
     if (!have) continue;
 
@@ -716,10 +678,9 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
     bool ndn = false;
     if (own) {
 #pragma unroll
-      for (int f = 0; f < NS; ++f) nst[f] = tape[((H - 1) * TCH + f) * GT + G.r];
-      ndn = tape[((H - 1) * TCH + NS) * GT + G.r] != 0.f;
+      for (int f = 0; f < NS; ++f) nst[f] = tape[((H - 1) * TCH + f) * GT + G.row];
+      ndn = tape[((H - 1) * TCH + NS) * GT + G.row] != 0.f;
     }
-    bool dx_pending = false, dx_add = false;
     for (int k = H - 1; k >= 0; --k) {
       float zt[MAXA];
       const bool dnk = ndn;
@@ -730,27 +691,20 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
       if (own) {
 #pragma unroll
         for (int j = 0; j < MAXA; ++j)
-          if (j < P.out) zt[j] = tape[(k * TCH + NS + 1 + j) * GT + G.r];
+          if (j < P.out) zt[j] = tape[(k * TCH + NS + 1 + j) * GT + G.row];
       }
-      layer1_issue<NS>(G, P, st, (float)(k + 1));     // recompute of step k's layer 1
-      if (own && dx_pending) {                        // input gradient of step k + 1
-        float dxn[16];
-        collect_dx(G, dxn);
-        if (dx_add) {
-#pragma unroll
-          for (int f = 0; f < NS; ++f)
-            if (f < obs_dim) lam[f] += dxn[f];
-        }
-      }
+      float d1[32], a1p[32];
+      put_x<NS>(G, G.X(k), P, st, (float)(k + 1));
+      layer1_issue(G, P, G.X(k), d1);                // recompute of step k's layer 1, overlapped with the adjoint
       float zb[MAXA];
 #pragma unroll
       for (int j = 0; j < MAXA; ++j) zb[j] = 0.f;
-      const bool active = own && valid && (p.mask_at_done ? !dnk : true);
+      const bool active = valid && (p.mask_at_done ? !dnk : true);
       if (own) {
         if (k > 0) {
 #pragma unroll
-          for (int f = 0; f < NS; ++f) nst[f] = tape[((k - 1) * TCH + f) * GT + G.r];
-          ndn = tape[((k - 1) * TCH + NS) * GT + G.r] != 0.f;
+          for (int f = 0; f < NS; ++f) nst[f] = tape[((k - 1) * TCH + f) * GT + G.row];
+          ndn = tape[((k - 1) * TCH + NS) * GT + G.row] != 0.f;
         }
         if (active) {
           float a[MAXA], g[MAXA], abar[MAXA];
@@ -804,54 +758,56 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           for (int j = 0; j < MAXA; ++j) zb[j] = abar[j] * g[j];
         }
       }
-      layer1_finish<true, AF>(G, P, 0, G.h == 0 ? 0 : 4);      // the helper converts the whole row meanwhile
+      layer1_finish<true, AF>(G, P, d1, a1p);
       layer2_back<true, false, AF>(G, P, zb, nullptr, acc3);
-      backprop<true>(G, P, k > 0, part);
-      dx_pending = k > 0;
-      dx_add = active && k > 0;
+      float dx[NS];
+      backprop<true, NS>(G, P, k > 0, part, G.X(k), a1p, dx);
+      if (active && k > 0) {                          // + the policy's input gradient of step k
+#pragma unroll
+        for (int f = 0; f < NS; ++f)
+          if (f < obs_dim) lam[f] += dx[f];
+      }
     }
+    wg::wg_sync(G.g);                                 // step 0's dW1 product has read its observation planes
   }
 
-  // ============================ per-group partials ============================
-  group_sync(G.g);
+  // ============================ per-warpgroup partials ============================
+  wg::wg_sync(G.g);
+  const int lane = G.t & 31, w4 = G.t >> 5;
   if (alg != ALG_TRACE) {
     const NetL& U = (alg == ALG_PEV) ? V : P;
-    const int lane = G.r & 31, wq = G.wg & 3;
     constexpr int stride = MAXA * 64 + MAXA;
-    float* rg = reinterpret_cast<float*>(G.P);                         // [4 quarters][stride]: the planes are dead
-    if ((lane & 1) == 0) {
+    float* rg = reinterpret_cast<float*>(G.P);                         // [4 warps][stride]: the planes are dead
 #pragma unroll
-      for (int a = 0; a < MAXA; ++a)
-        if (a < U.out) {
-          rg[wq * stride + a * 64 + 32 * G.h + tcf::col16(lane)] = acc3.w0[a];
-          rg[wq * stride + a * 64 + 32 * G.h + 16 + tcf::col16(lane)] = acc3.w1[a];
-        }
-    }
-    if (own && lane == 0) {
+    for (int a = 0; a < MAXA; ++a)
+      if (a < U.out) {
+        const int col = 8 * (lane >> 2) + 2 * G.c;
+        rg[w4 * stride + a * 64 + col] = acc3.w[a][0];
+        rg[w4 * stride + a * 64 + col + 1] = acc3.w[a][1];
+        float sb = acc3.b[a];                                          // owners' rows; 0 elsewhere
 #pragma unroll
-      for (int a = 0; a < MAXA; ++a)
-        if (a < U.out) rg[wq * stride + MAXA * 64 + a] = acc3.b[a];
-    }
-    group_sync(G.g);
-    const int t = G.h * GT + G.r;
-    for (int i = t; i < U.out * 64; i += GTH) {
+        for (int o = 16; o > 0; o >>= 1) sb += __shfl_xor_sync(0xffffffffu, sb, o);
+        if (lane == 0) rg[w4 * stride + MAXA * 64 + a] = sb;
+      }
+    wg::wg_sync(G.g);
+    for (int i = G.t; i < U.out * 64; i += 128) {
       const int a = i >> 6, j = i & 63;
       part[U.g_w3 + i] = (rg[a * 64 + j] + rg[stride + a * 64 + j]) + (rg[2 * stride + a * 64 + j] + rg[3 * stride + a * 64 + j]);
     }
-    if (t < U.out)
-      part[U.g_b3 + t] = (rg[MAXA * 64 + t] + rg[stride + MAXA * 64 + t]) +
-                         (rg[2 * stride + MAXA * 64 + t] + rg[3 * stride + MAXA * 64 + t]);
-    group_sync(G.g);
+    if (G.t < U.out)
+      part[U.g_b3 + G.t] = (rg[MAXA * 64 + G.t] + rg[stride + MAXA * 64 + G.t]) +
+                           (rg[2 * stride + MAXA * 64 + G.t] + rg[3 * stride + MAXA * 64 + G.t]);
+    wg::wg_sync(G.g);
   }
-  {  // the three scalars of the group (fixed order; only owner threads carry values)
+  {  // the three scalars of the sub-tile slot (fixed order over its 64 rows; only owner threads carry values)
     float* sc = reinterpret_cast<float*>(G.P);
-    if (own) { sc[G.r] = loss_acc; sc[GT + G.r] = vmean_acc; sc[2 * GT + G.r] = done_acc; }
-    group_sync(G.g);
-    if (own && G.r < 3) {
+    if (own) { sc[G.row] = loss_acc; sc[GT + G.row] = vmean_acc; sc[2 * GT + G.row] = done_acc; }
+    wg::wg_sync(G.g);
+    if (G.t < 3) {
       const int nparam = (alg == ALG_PEV) ? V.nparam : P.nparam;
       float s = 0.f;
-      for (int i = 0; i < GT; ++i) s += sc[G.r * GT + i];
-      part[nparam + G.r] = s;
+      for (int i = 0; i < GT; ++i) s += sc[G.t * GT + i];
+      part[nparam + G.t] = s;
     }
   }
 }
