@@ -9,24 +9,13 @@
 #include <stdlib.h>
 #include <string.h>
 
-#include <atomic>
 #include <new>
 #include <string>
 
 #include "dense_tc.cuh"
+#include "host_util.h"
 
 using namespace gops;
-
-namespace gops {
-int dense_fail(const std::string& msg);       // defined in gops_b200.cu (thread-local last error)
-void dense_count_launch(int n);
-}  // namespace gops
-
-#define DCUDA(expr)                                                                              \
-  do {                                                                                           \
-    cudaError_t e__ = (expr);                                                                    \
-    if (e__ != cudaSuccess) return gops::dense_fail(std::string(#expr) + ": " + cudaGetErrorString(e__)); \
-  } while (0)
 
 constexpr int kMaxLayers = 8, kMaxSlots = 128, kMaxWidth = 256;
 
@@ -53,37 +42,20 @@ struct gops_b200_mlpnet {
   float* wpart = nullptr;
   float* bpart = nullptr;
   int wchunks = 1;
-  bool attr_set = false;
 };
 
 namespace {
 
-struct DevGuard2 {
-  int prev = -1;
-  bool sw = false;
-  explicit DevGuard2(int dev) {
-    if (cudaGetDevice(&prev) == cudaSuccess && prev != dev) sw = cudaSetDevice(dev) == cudaSuccess;
-  }
-  ~DevGuard2() {
-    if (sw) cudaSetDevice(prev);
-  }
-};
-
 template <int EPI, bool GRAD>
 int launch_gemm(gops_b200_mlpnet* net, const dense::GemmArgs& a, cudaStream_t st) {
   const size_t smem = dense::gemm_smem(a.n, GRAD);
-  static bool attr_of[64] = {};        // per template instantiation and device: the widest tile (N = 128)
-  bool& attr = attr_of[net->device & 63];
-  if (!attr) {
-    DCUDA(cudaFuncSetAttribute(dense::dense_gemm_kernel<EPI, GRAD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)dense::gemm_smem(dense::NCMAX, GRAD)));
-    attr = true;
-  }
+  // the widest tile (N = 128)
+  if (allow_smem((const void*)dense::dense_gemm_kernel<EPI, GRAD>, net->device, (int)dense::gemm_smem(dense::NCMAX, GRAD)))
+    return 1;
   dim3 grid((unsigned)((a.rows + dense::TM - 1) / dense::TM), (unsigned)dense::splits_of(a.n));
   dense::dense_gemm_kernel<EPI, GRAD><<<grid, dense::NTH, smem, st>>>(a);
-  gops::dense_count_launch(1);
-  DCUDA(cudaGetLastError());
-  (void)net;
+  g_launches += 1;
+  CUDA_OK(cudaGetLastError());
   return 0;
 }
 
@@ -93,40 +65,22 @@ template <int EPI, bool GRAD>
 int launch_gemm_n(gops_b200_mlpnet* const* nets, int nn, const dense::GemmArgs* a, cudaStream_t st) {
   if (nn == 1) return launch_gemm<EPI, GRAD>(nets[0], a[0], st);
   const size_t smem = dense::gemm_smem(a[0].n, GRAD);
-  static bool attr_of[64] = {};
-  bool& attr = attr_of[nets[0]->device & 63];
-  if (!attr) {
-    DCUDA(cudaFuncSetAttribute(dense::dense_gemm_pair_kernel<EPI, GRAD>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)dense::gemm_smem(dense::NCMAX, GRAD)));
-    attr = true;
-  }
+  if (allow_smem((const void*)dense::dense_gemm_pair_kernel<EPI, GRAD>, nets[0]->device,
+                 (int)dense::gemm_smem(dense::NCMAX, GRAD)))
+    return 1;
   dense::GemmPair p;
   p.g[0] = a[0];
   p.g[1] = a[1];
   dim3 grid((unsigned)((a[0].rows + dense::TM - 1) / dense::TM), (unsigned)dense::splits_of(a[0].n), 2u);
   dense::dense_gemm_pair_kernel<EPI, GRAD><<<grid, dense::NTH, smem, st>>>(p);
-  gops::dense_count_launch(1);
-  DCUDA(cudaGetLastError());
+  g_launches += 1;
+  CUDA_OK(cudaGetLastError());
   return 0;
 }
 
 int set_wgrad_attr(gops_b200_mlpnet* const* nets, int nn) {
-  if (nn == 1) {
-    if (!nets[0]->attr_set) {
-      DCUDA(cudaFuncSetAttribute(dense::dense_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)dense::wgrad_smem()));
-      nets[0]->attr_set = true;
-    }
-    return 0;
-  }
-  static bool attr_of[64] = {};
-  bool& attr = attr_of[nets[0]->device & 63];
-  if (!attr) {
-    DCUDA(cudaFuncSetAttribute(dense::dense_wgrad_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)dense::wgrad_smem()));
-    attr = true;
-  }
-  return 0;
+  return allow_smem(nn == 1 ? (const void*)dense::dense_wgrad_kernel : (const void*)dense::dense_wgrad_pair_kernel,
+                    nets[0]->device, (int)dense::wgrad_smem());
 }
 
 // Forward pass of `nn` (1 or 2) networks of identical shape on the same input x; network i writes y[i].
@@ -217,8 +171,8 @@ int backward_n(gops_b200_mlpnet* const* nets, int nn, const float* const* dy, in
         dense::dense_reduce_pair_kernel<<<dim3((unsigned)((n + 255) / 256), 1u, 2u), 256, 0, st>>>(
             a->bpart, b->bpart, brows, n, grad[0] + a->b_off[l], grad[1] + b->b_off[l], accumulate);
       }
-      gops::dense_count_launch(4);
-      DCUDA(cudaGetLastError());
+      g_launches += 4;
+      CUDA_OK(cudaGetLastError());
     }
     if (l > 0 || dx[0]) {
       dense::GemmArgs a[2];
@@ -252,14 +206,14 @@ int backward_n(gops_b200_mlpnet* const* nets, int nn, const float* const* dy, in
 // Two handles may run as a pair when their shapes, activation, max_batch and slots agree and both are packed on
 // the same device.
 int check_pair(const gops_b200_mlpnet* a, const gops_b200_mlpnet* b, const char* fn) {
-  if (!a || !b) return dense_fail(std::string(fn) + ": null network handle");
-  if (a == b) return dense_fail(std::string(fn) + ": the two networks of a pair must be distinct handles");
+  if (!a || !b) return fail(std::string(fn) + ": null network handle");
+  if (a == b) return fail(std::string(fn) + ": the two networks of a pair must be distinct handles");
   bool same = a->nl == b->nl && a->act == b->act && a->max_batch == b->max_batch && a->slots == b->slots &&
               a->device == b->device;
   for (int l = 0; same && l <= a->nl; ++l) same = a->sizes[l] == b->sizes[l];
   if (!same)
-    return dense_fail(std::string(fn) + ": the two networks differ in layer sizes, activation, max_batch, slots or device");
-  if (!a->params || !b->params) return dense_fail(std::string(fn) + " before mlpnet_pack of both networks");
+    return fail(std::string(fn) + ": the two networks differ in layer sizes, activation, max_batch, slots or device");
+  if (!a->params || !b->params) return fail(std::string(fn) + " before mlpnet_pack of both networks");
   return 0;
 }
 
@@ -269,20 +223,20 @@ extern "C" {
 
 int gops_b200_mlpnet_create(const int32_t* sizes, int32_t n_sizes, int32_t hidden_act, int64_t max_batch, int32_t slots,
                             gops_b200_mlpnet** out) {
-  if (!sizes || !out || n_sizes < 2 || n_sizes > kMaxLayers + 1) return dense_fail("mlpnet: 1..8 layers");
-  if (max_batch < 1 || slots < 1 || slots > kMaxSlots) return dense_fail("mlpnet: bad max_batch / slots");
-  if (hidden_act < 0 || hidden_act > GOPS_ACT_LINEAR) return dense_fail("mlpnet: bad activation");
+  if (!sizes || !out || n_sizes < 2 || n_sizes > kMaxLayers + 1) return fail("mlpnet: 1..8 layers");
+  if (max_batch < 1 || slots < 1 || slots > kMaxSlots) return fail("mlpnet: bad max_batch / slots");
+  if (hidden_act < 0 || hidden_act > GOPS_ACT_LINEAR) return fail("mlpnet: bad activation");
   for (int i = 0; i < n_sizes; ++i)
-    if (sizes[i] < 1 || sizes[i] > kMaxWidth) return dense_fail("mlpnet: layer widths must be in 1..256");
+    if (sizes[i] < 1 || sizes[i] > kMaxWidth) return fail("mlpnet: layer widths must be in 1..256");
   *out = nullptr;
   gops_b200_mlpnet* net = new (std::nothrow) gops_b200_mlpnet();
-  if (!net) return dense_fail("out of host memory");
+  if (!net) return fail("out of host memory");
   cudaDeviceProp prop;
   if (cudaGetDevice(&net->device) != cudaSuccess || cudaGetDeviceProperties(&prop, net->device) != cudaSuccess) {
     delete net;
-    return dense_fail("no CUDA device");
+    return fail("no CUDA device");
   }
-  if (prop.major != 9 || prop.minor != 0) { delete net; return dense_fail("gops_b200 is built for sm_90a and needs an H100-class (sm_90) device"); }
+  if (prop.major != 9 || prop.minor != 0) { delete net; return fail("gops_b200 is built for sm_90a and needs an H100-class (sm_90) device"); }
   net->sm_count = prop.multiProcessorCount;
   net->max_smem = (int)prop.sharedMemPerBlockOptin;
   net->nl = n_sizes - 1;
@@ -315,7 +269,7 @@ int gops_b200_mlpnet_create(const int32_t* sizes, int32_t n_sizes, int32_t hidde
        cudaMalloc(&net->bpart, (size_t)64 * maxw * sizeof(float)) == cudaSuccess;
   if (!ok) {
     gops_b200_mlpnet_destroy(net);
-    return dense_fail("mlpnet: cudaMalloc failed");
+    return fail("mlpnet: cudaMalloc failed");
   }
   *out = net;
   return 0;
@@ -323,7 +277,7 @@ int gops_b200_mlpnet_create(const int32_t* sizes, int32_t n_sizes, int32_t hidde
 
 int gops_b200_mlpnet_destroy(gops_b200_mlpnet* net) {
   if (!net) return 0;
-  DevGuard2 dg(net->device);
+  DevGuard dg(net->device);
   for (int l = 0; l < kMaxLayers; ++l) { cudaFree(net->fwd_img[l]); cudaFree(net->bwd_img[l]); }
   for (int l = 0; l < kMaxLayers; ++l) { cudaFree(net->hbuf[l]); cudaFree(net->dbuf[l]); cudaFree(net->gbuf[l]); }
   cudaFree(net->delta[0]); cudaFree(net->delta[1]); cudaFree(net->wpart); cudaFree(net->bpart);
@@ -335,34 +289,34 @@ int gops_b200_mlpnet_destroy(gops_b200_mlpnet* net) {
 int64_t gops_b200_mlpnet_param_count(const gops_b200_mlpnet* net) { return net ? net->nparam : -1; }
 
 int gops_b200_mlpnet_pack(gops_b200_mlpnet* net, const float* params, void* stream) {
-  if (!net || !params) return dense_fail("null argument");
-  DevGuard2 dg(net->device);
+  if (!net || !params) return fail("null argument");
+  DevGuard dg(net->device);
   cudaStream_t st = (cudaStream_t)stream;
   for (int l = 0; l < net->nl; ++l) {
     dense::pack_dense_kernel<<<64, 256, 0, st>>>(params + net->w_off[l], net->sizes[l + 1], net->sizes[l], net->fwd_img[l],
                                                  net->bwd_img[l]);
-    gops::dense_count_launch(1);
+    g_launches += 1;
   }
-  DCUDA(cudaGetLastError());
+  CUDA_OK(cudaGetLastError());
   net->params = params;
   return 0;
 }
 
 int gops_b200_mlpnet_forward(gops_b200_mlpnet* net, const float* x, int32_t ldx, int64_t batch, int32_t slot, int32_t train,
                              float* y, int32_t ldy, void* stream) {
-  if (!net || !x || !y) return dense_fail("null argument");
-  if (!net->params) return dense_fail("mlpnet_forward before mlpnet_pack");
-  if (batch < 1 || batch > net->max_batch || slot < 0 || slot >= net->slots) return dense_fail("mlpnet_forward: bad batch / slot");
-  DevGuard2 dg(net->device);
+  if (!net || !x || !y) return fail("null argument");
+  if (!net->params) return fail("mlpnet_forward before mlpnet_pack");
+  if (batch < 1 || batch > net->max_batch || slot < 0 || slot >= net->slots) return fail("mlpnet_forward: bad batch / slot");
+  DevGuard dg(net->device);
   return forward_n(&net, 1, x, ldx, batch, slot, train, &y, ldy, (cudaStream_t)stream);
 }
 
 int gops_b200_mlpnet_backward(gops_b200_mlpnet* net, const float* dy, int32_t lddy, int64_t batch, int32_t slot,
                               float* grad_flat, int32_t accumulate, float* dx, int32_t lddx, void* stream) {
-  if (!net || !dy) return dense_fail("null argument");
+  if (!net || !dy) return fail("null argument");
   if (batch < 1 || batch > net->max_batch || slot < 0 || slot >= net->slots || !net->xin[slot])
-    return dense_fail("mlpnet_backward: no forward pass recorded in this slot");
-  DevGuard2 dg(net->device);
+    return fail("mlpnet_backward: no forward pass recorded in this slot");
+  DevGuard dg(net->device);
   return backward_n(&net, 1, &dy, lddy, batch, slot, &grad_flat, accumulate, &dx, lddx, (cudaStream_t)stream);
 }
 
@@ -370,10 +324,10 @@ int gops_b200_mlpnet_pair_forward(gops_b200_mlpnet* net_a, gops_b200_mlpnet* net
                                   int64_t batch, int32_t slot, int32_t train, float* y_a, float* y_b, int32_t ldy,
                                   void* stream) {
   if (check_pair(net_a, net_b, "mlpnet_pair_forward")) return 1;
-  if (!x || !y_a || !y_b) return dense_fail("mlpnet_pair_forward: null argument");
+  if (!x || !y_a || !y_b) return fail("mlpnet_pair_forward: null argument");
   if (batch < 1 || batch > net_a->max_batch || slot < 0 || slot >= net_a->slots)
-    return dense_fail("mlpnet_pair_forward: bad batch / slot");
-  DevGuard2 dg(net_a->device);
+    return fail("mlpnet_pair_forward: bad batch / slot");
+  DevGuard dg(net_a->device);
   gops_b200_mlpnet* nets[2] = {net_a, net_b};
   float* ys[2] = {y_a, y_b};
   return forward_n(nets, 2, x, ldx, batch, slot, train, ys, ldy, (cudaStream_t)stream);
@@ -383,12 +337,12 @@ int gops_b200_mlpnet_pair_backward(gops_b200_mlpnet* net_a, gops_b200_mlpnet* ne
                                    int32_t lddy, int64_t batch, int32_t slot, float* grad_a, float* grad_b,
                                    int32_t accumulate, float* dx_a, float* dx_b, int32_t lddx, void* stream) {
   if (check_pair(net_a, net_b, "mlpnet_pair_backward")) return 1;
-  if (!dy_a || !dy_b) return dense_fail("mlpnet_pair_backward: null argument");
+  if (!dy_a || !dy_b) return fail("mlpnet_pair_backward: null argument");
   if (!grad_a != !grad_b || !dx_a != !dx_b)
-    return dense_fail("mlpnet_pair_backward: grad_a / grad_b and dx_a / dx_b must both be set or both be NULL");
+    return fail("mlpnet_pair_backward: grad_a / grad_b and dx_a / dx_b must both be set or both be NULL");
   if (batch < 1 || batch > net_a->max_batch || slot < 0 || slot >= net_a->slots || !net_a->xin[slot] || !net_b->xin[slot])
-    return dense_fail("mlpnet_pair_backward: no forward pass recorded in this slot");
-  DevGuard2 dg(net_a->device);
+    return fail("mlpnet_pair_backward: no forward pass recorded in this slot");
+  DevGuard dg(net_a->device);
   gops_b200_mlpnet* nets[2] = {net_a, net_b};
   const float* dys[2] = {dy_a, dy_b};
   float* grads[2] = {grad_a, grad_b};
@@ -399,12 +353,12 @@ int gops_b200_mlpnet_pair_backward(gops_b200_mlpnet* net_a, gops_b200_mlpnet* ne
 /* Keep the per-layer deltas of every backward pass in its slot (memory: slots x max_batch x width per hidden layer) so
  * that mlpnet_wgrad_slots can contract the weight gradients over ALL slots at once. */
 int gops_b200_mlpnet_keep_deltas(gops_b200_mlpnet* net, int32_t enable) {
-  if (!net) return dense_fail("null argument");
-  DevGuard2 dg(net->device);
+  if (!net) return fail("null argument");
+  DevGuard dg(net->device);
   if (enable && !net->gbuf[0]) {
     for (int l = 0; l + 1 < net->nl; ++l) {
       const size_t per = (size_t)net->max_batch * net->sizes[l + 1];
-      DCUDA(cudaMalloc(&net->gbuf[l], per * net->slots * sizeof(float)));
+      CUDA_OK(cudaMalloc(&net->gbuf[l], per * net->slots * sizeof(float)));
       for (int s = 0; s < net->slots; ++s) net->gl[s][l] = net->gbuf[l] + per * s;
     }
   }
@@ -418,16 +372,13 @@ int gops_b200_mlpnet_keep_deltas(gops_b200_mlpnet* net, int32_t enable) {
 int gops_b200_mlpnet_wgrad_slots(gops_b200_mlpnet* net, int32_t slot0, int32_t nslots, int64_t batch, const float* x,
                                  int32_t ldx, int64_t x_stride, const float* dy, int32_t lddy, int64_t dy_stride,
                                  float* grad_flat, int32_t accumulate, void* stream) {
-  if (!net || !x || !dy || !grad_flat) return dense_fail("null argument");
-  if (!net->keep_deltas) return dense_fail("mlpnet_wgrad_slots needs mlpnet_keep_deltas(1)");
+  if (!net || !x || !dy || !grad_flat) return fail("null argument");
+  if (!net->keep_deltas) return fail("mlpnet_wgrad_slots needs mlpnet_keep_deltas(1)");
   if (slot0 < 0 || nslots < 1 || slot0 + nslots > net->slots || batch < 1 || batch > net->max_batch)
-    return dense_fail("mlpnet_wgrad_slots: bad slot range / batch");
-  DevGuard2 dg(net->device);
+    return fail("mlpnet_wgrad_slots: bad slot range / batch");
+  DevGuard dg(net->device);
   cudaStream_t st = (cudaStream_t)stream;
-  if (!net->attr_set) {
-    DCUDA(cudaFuncSetAttribute(dense::dense_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dense::wgrad_smem()));
-    net->attr_set = true;
-  }
+  if (set_wgrad_attr(&net, 1)) return 1;
   for (int l = net->nl - 1; l >= 0; --l) {
     const int n = net->sizes[l + 1], k = net->sizes[l];
     dense::WgradArgs w;
@@ -451,8 +402,8 @@ int gops_b200_mlpnet_wgrad_slots(gops_b200_mlpnet* net, int32_t slot0, int32_t n
                                                                                                    net->bpart, rpb, nslots, w.sy);
     dense::dense_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(net->bpart, brows, n, grad_flat + net->b_off[l],
                                                                           accumulate);
-    gops::dense_count_launch(4);
-    DCUDA(cudaGetLastError());
+    g_launches += 4;
+    CUDA_OK(cudaGetLastError());
   }
   return 0;
 }

@@ -11,30 +11,14 @@
 #include <string>
 
 #include "dsac_common.cuh"
+#include "host_util.h"
 
-namespace gops {
-int dense_fail(const std::string& msg);
-void dense_count_launch(int n);
-}  // namespace gops
+using gops::DevGuard;
+using gops::fail;
 
 namespace {
 
 using namespace gops::dsac;
-
-struct DevGuard3 {
-  int prev = -1;
-  bool sw = false;
-  explicit DevGuard3(const void* p) {
-    cudaPointerAttributes a;
-    int dev = -1;
-    if (p && cudaPointerGetAttributes(&a, p) == cudaSuccess && a.type == cudaMemoryTypeDevice) dev = a.device;
-    (void)cudaGetLastError();
-    if (dev >= 0 && cudaGetDevice(&prev) == cudaSuccess && prev != dev) sw = cudaSetDevice(dev) == cudaSuccess;
-  }
-  ~DevGuard3() {
-    if (sw) cudaSetDevice(prev);
-  }
-};
 
 // StochaPolicy head (mlp.py:203-221, std_type "mlp_shared") + TanhGaussDistribution.rsample (:37-50):
 //   mean | log_std = logits;  std = exp(clamp(log_std, lo, hi));  u = mean + std eps;  a = half tanh(u) + mid
@@ -137,36 +121,30 @@ __global__ void dsac_policy_loss_kernel(const float* __restrict__ qo, const floa
 
 }  // namespace
 
-#define KCHECK()                                                                                      \
-  do {                                                                                                \
-    cudaError_t e__ = cudaGetLastError();                                                             \
-    if (e__ != cudaSuccess) return gops::dense_fail(std::string("dsac kernel: ") + cudaGetErrorString(e__)); \
-  } while (0)
-
 extern "C" {
 
 int gops_b200_dsac_sample(const float* logits, const float* eps, int64_t batch, int32_t act_dim, float min_log_std,
                           float max_log_std, const float* act_half, const float* act_mid, float* act, float* logp,
                           const float* obs, int32_t obs_dim, float* qin, int32_t ldq, float* stats, void* stream) {
   if (!logits || !eps || !act || !logp || !act_half || !act_mid || batch < 1 || act_dim < 1)
-    return gops::dense_fail("dsac_sample: bad argument");
-  DevGuard3 dg(logits);
+    return fail("dsac_sample: bad argument");
+  DevGuard dg(logits);
   dsac_sample_kernel<<<(unsigned)((batch + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
       logits, eps, batch, act_dim, min_log_std, max_log_std, act_half, act_mid, act, logp, obs, obs_dim, qin, ldq, stats);
-  gops::dense_count_launch(1);
-  KCHECK();
+  gops::g_launches += 1;
+  CUDA_OK(cudaGetLastError(), "dsac kernel");
   return 0;
 }
 
 int gops_b200_dsac_sample_backward(const float* logits, const float* eps, int64_t batch, int32_t act_dim, float min_log_std,
                                    float max_log_std, const float* act_half, const float* d_act, int32_t ldda,
                                    int32_t act_col0, float logp_coeff, float* d_logits, void* stream) {
-  if (!logits || !eps || !d_act || !d_logits || !act_half || batch < 1) return gops::dense_fail("dsac_sample_backward: bad argument");
-  DevGuard3 dg(logits);
+  if (!logits || !eps || !d_act || !d_logits || !act_half || batch < 1) return fail("dsac_sample_backward: bad argument");
+  DevGuard dg(logits);
   dsac_sample_bwd_kernel<<<(unsigned)((batch + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
       logits, eps, batch, act_dim, min_log_std, max_log_std, act_half, d_act, ldda, act_col0, logp_coeff, d_logits);
-  gops::dense_count_launch(1);
-  KCHECK();
+  gops::g_launches += 1;
+  CUDA_OK(cudaGetLastError(), "dsac kernel");
   return 0;
 }
 
@@ -174,23 +152,23 @@ int gops_b200_dsac_q_loss(const float* q_out, const float* q_next_out, const flo
                           const float* rew, const float* done, int64_t batch, float gamma, float alpha, int32_t bound,
                           float* d_q_out, float* out3, void* stream) {
   if (!q_out || !q_next_out || !z_next || !logp_next || !rew || !done || !d_q_out || !out3 || batch < 1)
-    return gops::dense_fail("dsac_q_loss: bad argument");
-  DevGuard3 dg(q_out);
+    return fail("dsac_q_loss: bad argument");
+  DevGuard dg(q_out);
   dsac_q_loss_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(q_out, q_next_out, z_next, logp_next, rew, done, batch, gamma, alpha,
                                                          bound, d_q_out, out3);
-  gops::dense_count_launch(1);
-  KCHECK();
+  gops::g_launches += 1;
+  CUDA_OK(cudaGetLastError(), "dsac kernel");
   return 0;
 }
 
 int gops_b200_dsac_policy_loss(const float* q_out, const float* logp_new, int64_t batch, float alpha, float target_entropy,
                                float* d_q_out, float* out5, const float* stats, void* stream) {
-  if (!q_out || !logp_new || !d_q_out || !out5 || batch < 1) return gops::dense_fail("dsac_policy_loss: bad argument");
-  DevGuard3 dg(q_out);
+  if (!q_out || !logp_new || !d_q_out || !out5 || batch < 1) return fail("dsac_policy_loss: bad argument");
+  DevGuard dg(q_out);
   dsac_policy_loss_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(q_out, logp_new, batch, alpha, target_entropy, d_q_out, out5,
                                                               stats);
-  gops::dense_count_launch(1);
-  KCHECK();
+  gops::g_launches += 1;
+  CUDA_OK(cudaGetLastError(), "dsac kernel");
   return 0;
 }
 

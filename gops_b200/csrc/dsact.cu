@@ -11,32 +11,16 @@
 #include <string>
 
 #include "dsac_common.cuh"
+#include "host_util.h"
 
-namespace gops {
-int dense_fail(const std::string& msg);
-void dense_count_launch(int n);
-}  // namespace gops
+using gops::DevGuard;
+using gops::fail;
 
 namespace {
 
 using namespace gops::dsac;
 
 constexpr float kBias = 0.1f;                    // dsact.py:286
-
-struct DevGuard4 {
-  int prev = -1;
-  bool sw = false;
-  explicit DevGuard4(const void* p) {
-    cudaPointerAttributes a;
-    int dev = -1;
-    if (p && cudaPointerGetAttributes(&a, p) == cudaSuccess && a.type == cudaMemoryTypeDevice) dev = a.device;
-    (void)cudaGetLastError();
-    if (dev >= 0 && cudaGetDevice(&prev) == cudaSuccess && prev != dev) sw = cudaSetDevice(dev) == cudaSuccess;
-  }
-  ~DevGuard4() {
-    if (sw) cudaSetDevice(prev);
-  }
-};
 
 // r + (1 - d) gamma (q - alpha logp), in the reference's operation order
 __device__ __forceinline__ float td_target(float r, float d, float gamma, float q, float alpha, float logp) {
@@ -153,12 +137,6 @@ __global__ void dsact_sample_bwd_kernel(const float* __restrict__ logits, const 
 
 }  // namespace
 
-#define KCHECK()                                                                                       \
-  do {                                                                                                 \
-    cudaError_t e__ = cudaGetLastError();                                                              \
-    if (e__ != cudaSuccess) return gops::dense_fail(std::string("dsact kernel: ") + cudaGetErrorString(e__)); \
-  } while (0)
-
 extern "C" {
 
 int gops_b200_dsact_q_loss(const float* q1_out, const float* q2_out, const float* q1_next_out, const float* q2_next_out,
@@ -167,13 +145,13 @@ int gops_b200_dsact_q_loss(const float* q1_out, const float* q2_out, const float
                            int32_t mean_std_unset, float* d_q1_out, float* d_q2_out, float* out9, void* stream) {
   if (!q1_out || !q2_out || !q1_next_out || !q2_next_out || !z1_next || !z2_next || !logp_next || !rew || !done ||
       !mean_std || !d_q1_out || !d_q2_out || !out9 || batch < 1)
-    return gops::dense_fail("dsact_q_loss: bad argument");
-  DevGuard4 dg(q1_out);
+    return fail("dsact_q_loss: bad argument");
+  DevGuard dg(q1_out);
   dsact_q_loss_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(q1_out, q2_out, q1_next_out, q2_next_out, z1_next, z2_next,
                                                           logp_next, rew, done, batch, gamma, alpha, (float)(1.0 - tau_b),
                                                           (float)tau_b, mean_std_unset, mean_std, d_q1_out, d_q2_out, out9);
-  gops::dense_count_launch(1);
-  KCHECK();
+  gops::g_launches += 1;
+  CUDA_OK(cudaGetLastError(), "dsact kernel");
   return 0;
 }
 
@@ -181,12 +159,12 @@ int gops_b200_dsact_policy_loss(const float* q1_out, const float* q2_out, const 
                                 float target_entropy, float* d_q1_out, float* d_q2_out, float* out5, const float* stats,
                                 void* stream) {
   if (!q1_out || !q2_out || !logp_new || !d_q1_out || !d_q2_out || !out5 || batch < 1)
-    return gops::dense_fail("dsact_policy_loss: bad argument");
-  DevGuard4 dg(q1_out);
+    return fail("dsact_policy_loss: bad argument");
+  DevGuard dg(q1_out);
   dsact_policy_loss_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(q1_out, q2_out, logp_new, batch, alpha, target_entropy,
                                                                d_q1_out, d_q2_out, out5, stats);
-  gops::dense_count_launch(1);
-  KCHECK();
+  gops::g_launches += 1;
+  CUDA_OK(cudaGetLastError(), "dsact kernel");
   return 0;
 }
 
@@ -195,13 +173,13 @@ int gops_b200_dsact_sample_backward(const float* logits, const float* eps, int64
                                     const float* d_act_2, int32_t ldda, int32_t act_col0, float logp_coeff,
                                     float* d_logits, void* stream) {
   if (!logits || !eps || !d_act_1 || !d_act_2 || !d_logits || !act_half || batch < 1 || act_dim < 1)
-    return gops::dense_fail("dsact_sample_backward: bad argument");
-  DevGuard4 dg(logits);
+    return fail("dsact_sample_backward: bad argument");
+  DevGuard dg(logits);
   dsact_sample_bwd_kernel<<<(unsigned)((batch + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
       logits, eps, batch, act_dim, min_log_std, max_log_std, act_half, d_act_1, d_act_2, ldda, act_col0, logp_coeff,
       d_logits);
-  gops::dense_count_launch(1);
-  KCHECK();
+  gops::g_launches += 1;
+  CUDA_OK(cudaGetLastError(), "dsact kernel");
   return 0;
 }
 

@@ -1,28 +1,11 @@
-// Instantiations of the fused rollout kernel for ModelVehConti (own translation unit: parallel build).
-#include "kernel.cuh"
+// Kernel table of ModelVehConti (own translation unit: parallel build).
+#include "model_kernels.cuh"
 
 namespace gops {
 
-typedef void (*RolloutFn)(const KParams);
-typedef void (*StepFn)(const KParams, const float*, int, float*, float*, float*);
-
-template <int ALG>
-static RolloutFn pick(int hid, int cfg) {
-  if (hid > 64) return rollout_kernel<ModelVehConti, 256, 32, 256, ALG>;
-  switch (cfg) {
-    case 0: return rollout_kernel<ModelVehConti, 64, 128, 512, ALG>;
-    case 1: return rollout_kernel<ModelVehConti, 64, 64, 256, ALG>;
-    default: return rollout_kernel<ModelVehConti, 64, 32, 128, ALG>;
-  }
-}
-
-RolloutFn rollout_fn_vehconti(int hid, int cfg, int alg) {
-  switch (alg) {
-    case ALG_FHADP: return pick<ALG_FHADP>(hid, cfg);
-    case ALG_PIM: return pick<ALG_PIM>(hid, cfg);
-    case ALG_PEV: return pick<ALG_PEV>(hid, cfg);
-    default: return pick<ALG_TRACE>(hid, cfg);
-  }
+const ModelKernels& kernels_vehconti() {
+  static const ModelKernels k = model_kernels<ModelVehConti, 0>();
+  return k;
 }
 
 }  // namespace gops

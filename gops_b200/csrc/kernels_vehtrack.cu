@@ -1,38 +1,14 @@
-// Instantiations of the fused rollout kernel for ModelVehTrack (own translation unit: parallel build).
-#include "kernel.cuh"
+// Kernel table of ModelVehTrack and the veh3dof_tracking_detour kernels (own translation unit: parallel build).
 #include "lw_rollout.cuh"
 #include "lw_detour.cuh"
+#include "model_kernels.cuh"
 
 namespace gops {
 
-typedef void (*RolloutFn)(const KParams);
-typedef void (*StepFn)(const KParams, const float*, int, float*, float*, float*);
-
-template <int ALG>
-static RolloutFn pick(int hid, int cfg) {
-  if (hid > 64) return rollout_kernel<ModelVehTrack, 256, 32, 256, ALG>;
-  switch (cfg) {
-    case 0: return rollout_kernel<ModelVehTrack, 64, 128, 512, ALG>;
-    case 1: return rollout_kernel<ModelVehTrack, 64, 64, 256, ALG>;
-    default: return rollout_kernel<ModelVehTrack, 64, 32, 128, ALG>;
-  }
-}
-
-RolloutFn rollout_fn_vehtrack(int hid, int cfg, int alg) {
-  switch (alg) {
-    case ALG_FHADP: return pick<ALG_FHADP>(hid, cfg);
-    case ALG_PIM: return pick<ALG_PIM>(hid, cfg);
-    case ALG_PEV: return pick<ALG_PEV>(hid, cfg);
-    default: return pick<ALG_TRACE>(hid, cfg);
-  }
-}
-
-LwFn lw_fn_vehtrack(int which) {   // layer-wise path of the wide nets: init / forward step / reverse step
-  switch (which) {
-    case 0: return lw_init_kernel<ModelVehTrack>;
-    case 1: return lw_step_kernel<ModelVehTrack>;
-    default: return lw_reverse_kernel<ModelVehTrack>;
-  }
+const ModelKernels& kernels_vehtrack() {
+  static const ModelKernels k = model_kernels<ModelVehTrack, 0>(
+      {lw_init_kernel<ModelVehTrack>, lw_step_kernel<ModelVehTrack>, lw_reverse_kernel<ModelVehTrack>});
+  return k;
 }
 
 LwFn lw_fn_vehtrack_detour(int which) {   // veh3dof_tracking_detour: forward step / reverse step (init is shared)

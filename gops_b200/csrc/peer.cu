@@ -24,10 +24,10 @@
 #include <new>
 #include <string>
 
-namespace gops {
-int dense_fail(const std::string& msg);
-void dense_count_launch(int n);
-}  // namespace gops
+#include "host_util.h"
+
+using gops::DevGuard;
+using gops::fail;
 
 namespace {
 
@@ -35,12 +35,6 @@ constexpr int kMaxWorld = 16;
 constexpr int kBlocks = 8;                 // CTAs per call; each owns a contiguous chunk and its own flags
 constexpr int kThreads = 256;
 constexpr long long kSpinLimitNs = 60000000000ll;    // 60 s: a peer that never arrives must not hang the GPU for good
-
-#define PCUDA(expr)                                                                                     \
-  do {                                                                                                  \
-    cudaError_t e__ = (expr);                                                                           \
-    if (e__ != cudaSuccess) return gops::dense_fail(std::string(#expr) + ": " + cudaGetErrorString(e__)); \
-  } while (0)
 
 struct PeerArgs {
   int world, rank;
@@ -126,17 +120,6 @@ __global__ void __launch_bounds__(kThreads) peer_allreduce_kernel(PeerArgs a) {
   }
 }
 
-struct PGuard {
-  int prev = -1;
-  bool sw = false;
-  explicit PGuard(int dev) {
-    if (dev >= 0 && cudaGetDevice(&prev) == cudaSuccess && prev != dev) sw = cudaSetDevice(dev) == cudaSuccess;
-  }
-  ~PGuard() {
-    if (sw) cudaSetDevice(prev);
-  }
-};
-
 }  // namespace
 
 struct gops_b200_peer {
@@ -150,27 +133,25 @@ struct gops_b200_peer {
   size_t region_bytes = 0;
 };
 
-using gops::dense_fail;
-
 extern "C" {
 
 int gops_b200_peer_create(int32_t world, int32_t rank, int64_t max_floats, gops_b200_peer** out) {
-  if (!out) return dense_fail("peer_create: null out");
+  if (!out) return fail("peer_create: null out");
   *out = nullptr;
-  if (world < 1 || world > kMaxWorld || rank < 0 || rank >= world) return dense_fail("peer_create: world must be 1..16, 0 <= rank < world");
-  if (max_floats < 1) return dense_fail("peer_create: max_floats must be positive");
+  if (world < 1 || world > kMaxWorld || rank < 0 || rank >= world) return fail("peer_create: world must be 1..16, 0 <= rank < world");
+  if (max_floats < 1) return fail("peer_create: max_floats must be positive");
   gops_b200_peer* p = new (std::nothrow) gops_b200_peer();
-  if (!p) return dense_fail("out of host memory");
+  if (!p) return fail("out of host memory");
   p->world = world;
   p->rank = rank;
   p->cap = (max_floats + 3) / 4 * 4;
-  if (cudaGetDevice(&p->device) != cudaSuccess) { delete p; return dense_fail("no CUDA device"); }
+  if (cudaGetDevice(&p->device) != cudaSuccess) { delete p; return fail("no CUDA device"); }
   p->region_bytes = flags_offset_floats(world, p->cap) * sizeof(float) + (size_t)2 * kBlocks * kMaxWorld * sizeof(unsigned) + 16;
   void* q = nullptr;
   if (cudaMalloc(&q, p->region_bytes) != cudaSuccess || cudaMemset(q, 0, p->region_bytes) != cudaSuccess) {
     cudaFree(q);
     delete p;
-    return dense_fail("peer_create: cudaMalloc of the exchange region failed");
+    return fail("peer_create: cudaMalloc of the exchange region failed");
   }
   p->base[rank] = static_cast<float*>(q);
   // the error word lives behind the flags
@@ -182,30 +163,30 @@ int gops_b200_peer_create(int32_t world, int32_t rank, int64_t max_floats, gops_
 }
 
 int gops_b200_peer_region_bytes(const gops_b200_peer* p, int64_t* bytes) {
-  if (!p || !bytes) return dense_fail("null argument");
+  if (!p || !bytes) return fail("null argument");
   *bytes = (int64_t)p->region_bytes;
   return 0;
 }
 
 int gops_b200_peer_export(gops_b200_peer* p, void* handle64) {
-  if (!p || !handle64) return dense_fail("null argument");
+  if (!p || !handle64) return fail("null argument");
   static_assert(sizeof(cudaIpcMemHandle_t) == GOPS_B200_IPC_HANDLE_BYTES, "handle size");
-  PGuard g(p->device);
+  DevGuard g(p->device);
   cudaIpcMemHandle_t h;
-  PCUDA(cudaIpcGetMemHandle(&h, p->base[p->rank]));
+  CUDA_OK(cudaIpcGetMemHandle(&h, p->base[p->rank]));
   memcpy(handle64, &h, sizeof(h));
   return 0;
 }
 
 int gops_b200_peer_connect(gops_b200_peer* p, const void* handles) {
-  if (!p || !handles) return dense_fail("null argument");
-  PGuard g(p->device);
+  if (!p || !handles) return fail("null argument");
+  DevGuard g(p->device);
   for (int r = 0; r < p->world; ++r) {
     if (r == p->rank) continue;
     cudaIpcMemHandle_t h;
     memcpy(&h, static_cast<const char*>(handles) + (size_t)r * GOPS_B200_IPC_HANDLE_BYTES, sizeof(h));
     void* q = nullptr;
-    PCUDA(cudaIpcOpenMemHandle(&q, h, cudaIpcMemLazyEnablePeerAccess));
+    CUDA_OK(cudaIpcOpenMemHandle(&q, h, cudaIpcMemLazyEnablePeerAccess));
     p->base[r] = static_cast<float*>(q);
     p->ipc_opened[r] = true;
   }
@@ -214,26 +195,26 @@ int gops_b200_peer_connect(gops_b200_peer* p, const void* handles) {
 }
 
 int gops_b200_peer_local_base(gops_b200_peer* p, void** base) {
-  if (!p || !base) return dense_fail("null argument");
+  if (!p || !base) return fail("null argument");
   *base = p->base[p->rank];
   return 0;
 }
 
 int gops_b200_peer_connect_local(gops_b200_peer* p, void* const* bases) {
-  if (!p || !bases) return dense_fail("null argument");
-  PGuard g(p->device);
+  if (!p || !bases) return fail("null argument");
+  DevGuard g(p->device);
   for (int r = 0; r < p->world; ++r) {
     if (r == p->rank) continue;
-    if (!bases[r]) return dense_fail("peer_connect_local: null region");
+    if (!bases[r]) return fail("peer_connect_local: null region");
     cudaPointerAttributes at;
-    PCUDA(cudaPointerGetAttributes(&at, bases[r]));
-    if (at.type != cudaMemoryTypeDevice) return dense_fail("peer_connect_local: not a device pointer");
+    CUDA_OK(cudaPointerGetAttributes(&at, bases[r]));
+    if (at.type != cudaMemoryTypeDevice) return fail("peer_connect_local: not a device pointer");
     if (at.device != p->device) {
       int can = 0;
-      PCUDA(cudaDeviceCanAccessPeer(&can, p->device, at.device));
-      if (!can) return dense_fail("peer_connect_local: no peer access between the devices");
+      CUDA_OK(cudaDeviceCanAccessPeer(&can, p->device, at.device));
+      if (!can) return fail("peer_connect_local: no peer access between the devices");
       const cudaError_t e = cudaDeviceEnablePeerAccess(at.device, 0);
-      if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) return dense_fail(std::string("cudaDeviceEnablePeerAccess: ") + cudaGetErrorString(e));
+      if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) return fail(std::string("cudaDeviceEnablePeerAccess: ") + cudaGetErrorString(e));
       (void)cudaGetLastError();
     }
     p->base[r] = static_cast<float*>(bases[r]);
@@ -244,11 +225,11 @@ int gops_b200_peer_connect_local(gops_b200_peer* p, void* const* bases) {
 
 int gops_b200_peer_allreduce(gops_b200_peer* p, float* buf, int64_t n, float* params, float* exp_avg, float* exp_avg_sq,
                              int64_t nparam, int32_t step, double lr, double beta1, double beta2, double eps, void* stream) {
-  if (!p || !buf) return dense_fail("null argument");
-  if (!p->connected) return dense_fail("peer_allreduce: peers are not connected");
-  if (n < 1 || n > p->cap) return dense_fail("peer_allreduce: vector longer than the exchange slots");
-  if (params && (!exp_avg || !exp_avg_sq || nparam < 1 || nparam > n || step < 1)) return dense_fail("peer_allreduce: bad Adam arguments");
-  PGuard g(p->device);
+  if (!p || !buf) return fail("null argument");
+  if (!p->connected) return fail("peer_allreduce: peers are not connected");
+  if (n < 1 || n > p->cap) return fail("peer_allreduce: vector longer than the exchange slots");
+  if (params && (!exp_avg || !exp_avg_sq || nparam < 1 || nparam > n || step < 1)) return fail("peer_allreduce: bad Adam arguments");
+  DevGuard g(p->device);
   PeerArgs a;
   memset(&a, 0, sizeof(a));
   a.world = p->world; a.rank = p->rank; a.cap = p->cap; a.seq = ++p->seq;
@@ -261,23 +242,23 @@ int gops_b200_peer_allreduce(gops_b200_peer* p, float* buf, int64_t n, float* pa
     a.step_size = (float)(lr / bc1); a.bc2_sqrt = (float)sqrt(bc2);
   }
   peer_allreduce_kernel<<<kBlocks, kThreads, 0, (cudaStream_t)stream>>>(a);
-  gops::dense_count_launch(1);
-  PCUDA(cudaGetLastError());
+  gops::g_launches += 1;
+  CUDA_OK(cudaGetLastError());
   return 0;
 }
 
 int gops_b200_peer_error(gops_b200_peer* p, int32_t* err) {
-  if (!p || !err) return dense_fail("null argument");
-  PGuard g(p->device);
+  if (!p || !err) return fail("null argument");
+  DevGuard g(p->device);
   unsigned e = 0;
-  PCUDA(cudaMemcpy(&e, p->err, sizeof(e), cudaMemcpyDeviceToHost));
+  CUDA_OK(cudaMemcpy(&e, p->err, sizeof(e), cudaMemcpyDeviceToHost));
   *err = (int32_t)e;
   return 0;
 }
 
 int gops_b200_peer_destroy(gops_b200_peer* p) {
   if (!p) return 0;
-  PGuard g(p->device);
+  DevGuard g(p->device);
   cudaDeviceSynchronize();
   for (int r = 0; r < p->world; ++r)
     if (p->ipc_opened[r]) cudaIpcCloseMemHandle(p->base[r]);
