@@ -206,10 +206,7 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
             float oc[6], ce, cl, ci;
             bool inf;
 #pragma unroll
-            for (int f = 0; f < 6; ++f) {
-              oc[f] = t.X[f * XS + col];
-              if (p.obs_scaling) oc[f] = oc[f] / p.osc[f] - p.osh[f];
-            }
+            for (int f = 0; f < 6; ++f) oc[f] = to_inner(p, f, t.X[f * XS + col]);
             cstr_eval(oc, ce, cl, ci, inf);
             cacc_a += (p.cstr_mode == 2 ? cl : ce) * p.gpow[k];
             cacc_b += ci * p.gpow[k];
@@ -217,82 +214,47 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
           }
         }
         if constexpr (M::KIND == 0) {
-          // state==obs models: `st` is the wrapper-level (outer) observation; ScaleObservation maps it to the
-          // model's inner state and back, ActionRepeat repeats the masked model step with the same action
+          // state==obs models: `st` is the wrapper-level (outer) observation
           if (valid) {
-            float in[NS];
+            wrapped_step<M>(p, obs_dim, st, a, active, r, dn);
 #pragma unroll
             for (int f = 0; f < NS; ++f)
-              in[f] = (p.obs_scaling && f < obs_dim) ? st[f] / p.osc[f] - p.osh[f] : st[f];
-            if (active) {
-              bool md = false;
-              const int reps = p.repeat_num > 0 ? p.repeat_num : 1;
-              float rsum = 0.f, rj = 0.f;
-              for (int j = 0; j < reps; ++j) {
-                M::step(p, in, a, rj, md);
-                rsum += rj;
-              }
-              r = (p.repeat_num > 0 && p.sum_reward) ? rsum : rj;
-              dn = md;
-            }
-#pragma unroll
-            for (int f = 0; f < NS; ++f) {
-              float o = (p.obs_scaling && f < obs_dim) ? (in[f] + p.osh[f]) * p.osc[f] : in[f];
-              if (p.clip_obs) o = fminf(fmaxf(o, p.obs_low[f]), p.obs_high[f]);
-              st[f] = o;
-              if (f < obs_dim) t.X[f * XS + col] = o;
-            }
+              if (f < obs_dim) t.X[f * XS + col] = st[f];
           }
-        }
-        if (M::KIND != 0 && active) {
-          bool md;
-          if constexpr (M::KIND == 0) {
+        } else if (active) {
+          const VehC vc = veh_const();
+          float o6[6];
+          if constexpr (M::KIND == 1) {
+#pragma unroll
+            for (int f = 0; f < 6; ++f) o6[f] = to_inner(p, f, t.X[f * XS + col]);
+            r = M::reward(o6, a);
+            veh_step(vc, st, a);
+            st[6] = st[6] + vc.dt;
+            const float tq = st[6] + p.veh_Pdt;
+            float* nr = const_cast<float*>(win.base) + (size_t)(k + p.veh_P + 1) * 4 * NT;
+            nr[0] = rt_x(p.rt, tq, path, spd);
+            nr[NT] = rt_y(p.rt, tq, path, spd);
+            nr[2 * NT] = rt_phi(p.rt, tq, path, spd);
+            nr[3 * NT] = rt_u(p.rt, tq, spd);
+            win.k0 = k + 1;
+            veh_write_obs<M::KIND, NT>(st, win, p.veh_P, t.X + col, XS, o6);
+            if (p.obs_scaling) veh_scale_obs(p, obs_dim, t.X + col, XS);
+            dn = M::done(o6);
           } else {
-            const VehC vc = veh_const();
-            float o6[6];
-            if constexpr (M::KIND == 1) {
-              // reward from the INCOMING observation (Veh3dofcontiModel.compute_reward :161-177)
-#pragma unroll
-              for (int f = 0; f < 6; ++f) {
-                o6[f] = t.X[f * XS + col];
-                if (p.obs_scaling) o6[f] = o6[f] / p.osc[f] - p.osh[f];
-              }
-              r = -(0.04f * (o6[0] * o6[0]) + 0.04f * (o6[1] * o6[1]) + 0.02f * (o6[2] * o6[2]) +
-                    0.02f * (o6[3] * o6[3]) + 0.01f * (o6[5] * o6[5]) + 0.01f * (a[0] * a[0]) + 0.01f * (a[1] * a[1]));
-              veh_step(vc, st, a);
-              st[6] = st[6] + vc.dt;
-              const float tq = st[6] + p.veh_Pdt;
-              float* nr = const_cast<float*>(win.base) + (size_t)(k + p.veh_P + 1) * 4 * NT;
-              nr[0] = rt_x(p.rt, tq, path, spd);
-              nr[NT] = rt_y(p.rt, tq, path, spd);
-              nr[2 * NT] = rt_phi(p.rt, tq, path, spd);
-              nr[3 * NT] = rt_u(p.rt, tq, spd);
-              win.k0 = k + 1;
-              veh_write_obs<M::KIND, NT>(st, win, p.veh_P, t.X + col, XS, o6);
-              if (p.obs_scaling) veh_scale_obs(p, obs_dim, t.X + col, XS);
-              md = (fabsf(o6[0]) > 10.f) || (fabsf(o6[1]) > 10.f) || (fabsf(o6[2]) > 3.14159265358979323846f);
-            } else {
-              // reward from the CURRENT state against reference[:, t] (veh3dof_tracking_model.py:59-73)
-              float q[4];
-              win.k0 = p.ref_t + k;
-              win.get(0, q);
-              const float ex = st[0] - q[0], ey = st[1] - q[1], ep = angle_normalize(st[2] - q[2]), eu = st[3] - q[3];
-              r = -(0.04f * (ex * ex) + 0.04f * (ey * ey) + 0.02f * (ep * ep) + 0.02f * (eu * eu) +
-                    0.01f * (st[5] * st[5]) + 0.01f * (a[0] * a[0]) + 0.01f * (a[1] * a[1]));
-              veh_step(vc, st, a);
-              win.k0 = p.ref_t + k + 1;
-              veh_write_obs<M::KIND, NT>(st, win, p.veh_P, t.X + col, XS, o6);
-              if (p.obs_scaling) veh_scale_obs(p, obs_dim, t.X + col, XS);
-              win.get(0, q);
-              md = (fabsf(st[0] - q[0]) > 5.f) || (fabsf(st[1] - q[1]) > 2.f) ||
-                   (fabsf(angle_normalize(st[2] - q[2])) > 3.14159265358979323846f);
-            }
+            float q[4];
+            win.k0 = p.ref_t + k;
+            win.get(0, q);
+            r = M::reward(st, q, a);
+            veh_step(vc, st, a);
+            win.k0 = p.ref_t + k + 1;
+            veh_write_obs<M::KIND, NT>(st, win, p.veh_P, t.X + col, XS, o6);
+            if (p.obs_scaling) veh_scale_obs(p, obs_dim, t.X + col, XS);
+            win.get(0, q);
+            dn = M::done(st, q);
           }
-          dn = md;
         }
         if (valid) {
-          // ShapingReward sits outside MaskAtDone: a masked (done) sample still pays (0 + shift) * scale
-          if (p.reward_shaping) r = (r + p.reward_shift) * p.reward_scale;
+          r = shape_reward(p, r);      // ShapingReward sits outside MaskAtDone: a masked sample pays (0 + shift) * scale
           vacc += r * p.gpow[k];
         }
         if (alg == ALG_TRACE && valid) {
@@ -426,7 +388,7 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
             if (p.obs_scaling) {
               veh_scale_obs(p, obs_dim, t.X + col, XS);
 #pragma unroll
-              for (int f = 0; f < 6; ++f) o6[f] = t.X[f * XS + col] / p.osc[f] - p.osh[f];   // as the forward sweep saw it
+              for (int f = 0; f < 6; ++f) o6[f] = to_inner(p, f, t.X[f * XS + col]);   // as the forward sweep saw it
             }
           } else {
             for (int f = 0; f < obs_dim; ++f) t.X[f * XS + col] = 0.f;
@@ -435,10 +397,7 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
           }
         } else {
 #pragma unroll
-          for (int f = 0; f < 6; ++f) {
-            o6[f] = t.X[f * XS + col];
-            if (p.obs_scaling) o6[f] = o6[f] / p.osc[f] - p.osh[f];
-          }
+          for (int f = 0; f < 6; ++f) o6[f] = to_inner(p, f, t.X[f * XS + col]);
         }
       }
       if (P.time_input) t.X[(P.in - 1) * XS + col] = (float)(k + 1);
@@ -455,70 +414,20 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
 #pragma unroll
           for (int j = 0; j < MAXA; ++j) z[j] = j < P.out ? tape[(k * TCH + NS + 1 + j) * NT + tid] : 0.f;
           process_action(p, P.out, z, a, g, nullptr);
-          const float rho = -p.gpow[k] * p.inv_B * (p.reward_shaping ? p.reward_scale : 1.f);
+          const float rho = reward_adjoint(p, k);
 #pragma unroll
           for (int j = 0; j < MAXA; ++j) abar[j] = 0.f;
           if constexpr (M::KIND == 0) {
-            // lam = adjoint of the OUTER observation obs_{k+1}.  Chain of step k:
-            //   obs_k -(1/scale, -shift)-> inner_0 -[model step x reps, same action]-> inner_reps
-            //         -(+shift, *scale)-> clip -> obs_{k+1}
-            const int reps = p.repeat_num > 0 ? p.repeat_num : 1;
-            float in0[NS], cur[NS];
-#pragma unroll
-            for (int f = 0; f < NS; ++f)
-              in0[f] = (p.obs_scaling && f < obs_dim) ? st[f] / p.osc[f] - p.osh[f] : st[f];
-            if (p.clip_obs) {            // clip passes gradient only where the raw next observation is inside
-              float rr;
-              bool md;
-#pragma unroll
-              for (int f = 0; f < NS; ++f) cur[f] = in0[f];
-              for (int j = 0; j < reps; ++j) M::step(p, cur, a, rr, md);
-#pragma unroll
-              for (int f = 0; f < NS; ++f) {
-                const float o = (p.obs_scaling && f < obs_dim) ? (cur[f] + p.osh[f]) * p.osc[f] : cur[f];
-                if (o < p.obs_low[f] || o > p.obs_high[f]) lam[f] = 0.f;
-              }
-            }
-            if (p.obs_scaling) {
-#pragma unroll
-              for (int f = 0; f < NS; ++f)
-                if (f < obs_dim) lam[f] *= p.osc[f];
-            }
-            for (int j = reps - 1; j >= 0; --j) {
-              float rr, aj[MAXA];
-              bool md;
-#pragma unroll
-              for (int f = 0; f < NS; ++f) cur[f] = in0[f];
-              for (int q = 0; q < j; ++q) M::step(p, cur, a, rr, md);      // state before repeat j
-              const float rho_j = (p.repeat_num == 0 || p.sum_reward || j == reps - 1) ? rho : 0.f;
-#pragma unroll
-              for (int q = 0; q < MAXA; ++q) aj[q] = 0.f;
-              M::step_bwd(p, cur, a, rho_j, lam, aj);
-#pragma unroll
-              for (int q = 0; q < MAXA; ++q) abar[q] += aj[q];
-            }
-            if (p.obs_scaling) {
-#pragma unroll
-              for (int f = 0; f < NS; ++f)
-                if (f < obs_dim) lam[f] /= p.osc[f];
-            }
+            wrapped_step_bwd<M>(p, obs_dim, st, a, rho, lam, abar);     // lam: adjoint of the outer observation obs_{k+1}
           } else {
             const VehC vc = veh_const();
             veh_step_bwd(vc, st, a, lam, abar);
-            abar[0] += rho * (-0.02f * a[0]);
-            abar[1] += rho * (-0.02f * a[1]);
             if constexpr (M::KIND == 1) {
-              ro6[0] = rho * (-0.08f * o6[0]); ro6[1] = rho * (-0.08f * o6[1]);
-              ro6[2] = rho * (-0.04f * o6[2]); ro6[3] = rho * (-0.04f * o6[3]);
-              ro6[5] = rho * (-0.02f * o6[5]);
+              M::reward_bwd(o6, a, rho, ro6, abar);
             } else {
               float q[4];
               win.get(0, q);
-              lam[0] += rho * (-0.08f * (st[0] - q[0]));
-              lam[1] += rho * (-0.08f * (st[1] - q[1]));
-              lam[2] += rho * (-0.04f * angle_normalize(st[2] - q[2]));
-              lam[3] += rho * (-0.04f * (st[3] - q[3]));
-              lam[5] += rho * (-0.02f * st[5]);
+              M::reward_bwd(st, q, a, rho, lam, abar);
             }
           }
 #pragma unroll
@@ -692,40 +601,21 @@ __global__ void model_step_kernel(const __grid_constant__ KParams p, const float
   const long long gs = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (gs >= p.batch) return;
   const int obs_dim = p.pol.obs;
-  float st[NS], old[NS], a[MAXA];
+  float st[NS], a[MAXA];
 #pragma unroll
-  for (int f = 0; f < NS; ++f) old[f] = st[f] = f < obs_dim ? p.obs[gs * obs_dim + f] : 0.f;
+  for (int f = 0; f < NS; ++f) st[f] = f < obs_dim ? p.obs[gs * obs_dim + f] : 0.f;
 #pragma unroll
   for (int j = 0; j < MAXA; ++j) {
     float gg = 1.f;
     a[j] = j < act_dim ? wrap_action(p, j, action[gs * act_dim + j], gg) : 0.f;
   }
-  const bool dn = p.done[gs] != 0.f;
+  bool dn = p.done[gs] != 0.f;
   float r = 0.f;
-  bool md = false;
-#pragma unroll
-  for (int f = 0; f < NS; ++f)
-    if (p.obs_scaling && f < obs_dim) st[f] = st[f] / p.osc[f] - p.osh[f];
-  if (!(p.mask_at_done && dn)) {
-    const int reps = p.repeat_num > 0 ? p.repeat_num : 1;
-    float rsum = 0.f, rj = 0.f;
-    for (int j = 0; j < reps; ++j) {
-      M::step(p, st, a, rj, md);
-      rsum += rj;
-    }
-    r = (p.repeat_num > 0 && p.sum_reward) ? rsum : rj;
-  }
-  (void)old;
-  if (p.mask_at_done) md = md || dn;
-  if (p.reward_shaping) r = (r + p.reward_shift) * p.reward_scale;
-#pragma unroll
-  for (int f = 0; f < NS; ++f) {
-    if (p.obs_scaling && f < obs_dim) st[f] = (st[f] + p.osh[f]) * p.osc[f];
-    if (p.clip_obs) st[f] = fminf(fmaxf(st[f], p.obs_low[f]), p.obs_high[f]);
-  }
+  wrapped_step<M>(p, obs_dim, st, a, !(p.mask_at_done && dn), r, dn);     // a masked sample stays done
+  r = shape_reward(p, r);
   for (int f = 0; f < obs_dim; ++f) next_obs[gs * obs_dim + f] = st[f];
   reward[gs] = r;
-  next_done[gs] = md ? 1.f : 0.f;
+  next_done[gs] = dn ? 1.f : 0.f;
 }
 
 
@@ -758,9 +648,8 @@ __global__ void veh_step_kernel(const __grid_constant__ KParams p, const float* 
   if (KIND == 1) {
     float o[6];
 #pragma unroll
-    for (int f = 0; f < 6; ++f) o[f] = p.obs_scaling ? obs[f] / p.osc[f] - p.osh[f] : obs[f];
-    r = -(0.04f * (o[0] * o[0]) + 0.04f * (o[1] * o[1]) + 0.02f * (o[2] * o[2]) + 0.02f * (o[3] * o[3]) +
-          0.01f * (o[5] * o[5]) + 0.01f * (a[0] * a[0]) + 0.01f * (a[1] * a[1]));
+    for (int f = 0; f < 6; ++f) o[f] = to_inner(p, f, obs[f]);
+    r = ModelVehConti::reward(o, a);
     veh_step(vc, s, a);
     const float nt = p.ref_time[gs] + vc.dt, tq = nt + p.veh_Pdt;
     const int path = (int)p.path_num[gs], spd = (int)p.u_num[gs];
@@ -778,33 +667,29 @@ __global__ void veh_step_kernel(const __grid_constant__ KParams p, const float* 
     w.base = nrp; w.k0 = 0;
     float o6[6];
     veh_write_obs<2, 1>(s, w, P, nobs, 1, o6);
-    md = (fabsf(o6[0]) > 10.f) || (fabsf(o6[1]) > 10.f) || (fabsf(o6[2]) > 3.14159265358979323846f);
+    md = ModelVehConti::done(o6);
   } else {
     RefWindow<2, 1> w;
     w.base = p.reference + gs * (size_t)p.ref_len * 4; w.k0 = p.ref_t;
     float q[4];
     w.get(0, q);
-    const float ex = s[0] - q[0], ey = s[1] - q[1], ep = angle_normalize(s[2] - q[2]), eu = s[3] - q[3];
-    r = -(0.04f * (ex * ex) + 0.04f * (ey * ey) + 0.02f * (ep * ep) + 0.02f * (eu * eu) + 0.01f * (s[5] * s[5]) +
-          0.01f * (a[0] * a[0]) + 0.01f * (a[1] * a[1]));
+    r = ModelVehTrack::reward(s, q, a);
     veh_step(vc, s, a);
     w.k0 = p.ref_t + 1;
     float o6[6];
     veh_write_obs<2, 1>(s, w, P, nobs, 1, o6);
     w.get(0, q);
-    md = (fabsf(s[0] - q[0]) > 5.f) || (fabsf(s[1] - q[1]) > 2.f) ||
-         (fabsf(angle_normalize(s[2] - q[2])) > 3.14159265358979323846f);
+    md = ModelVehTrack::done(s, q);
   }
 #pragma unroll
   for (int f = 0; f < 6; ++f) next_state[gs * 6 + f] = s[f];
   if (p.mask_at_done && dn) {     // MaskAtDone: frozen (inner) observation, zero reward
     r = 0.f;
-    for (int f = 0; f < obs_dim; ++f) nobs[f] = p.obs_scaling ? obs[f] / p.osc[f] - p.osh[f] : obs[f];
+    for (int f = 0; f < obs_dim; ++f) nobs[f] = to_inner(p, f, obs[f]);
   }
   if (p.mask_at_done) md = md || dn;
-  if (p.reward_shaping) r = (r + p.reward_shift) * p.reward_scale;
-  if (p.obs_scaling)
-    for (int f = 0; f < obs_dim; ++f) nobs[f] = (nobs[f] + p.osh[f]) * p.osc[f];
+  r = shape_reward(p, r);
+  if (p.obs_scaling) veh_scale_obs(p, obs_dim, nobs, 1);
   reward[gs] = r;
   next_done[gs] = md ? 1.f : 0.f;
 }

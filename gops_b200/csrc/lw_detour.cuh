@@ -117,7 +117,7 @@ __global__ void lw_step_detour_kernel(const __grid_constant__ KParams p, const _
                     (fabsf(angle_normalize(st[2] - q[2])) > 3.14159265358979323846f);
   if (p.pol.time_input) xn[obs_dim] = (float)(k + 2);
   for (int f = obs_dim + p.pol.time_input; f < a.ldx; ++f) xn[f] = 0.f;
-  if (p.reward_shaping) r = (r + p.reward_shift) * p.reward_scale;   // MaskAtDone sits inside ShapingReward (masked r = 0)
+  r = shape_reward(p, r);      // MaskAtDone sits inside ShapingReward (masked r = 0)
   a.vacc[b] += r * p.gpow[k];
   if (p.cstr_mode != 0) {
     const float pos = fmaxf(c, 0.f);
@@ -191,7 +191,7 @@ __global__ void lw_reverse_detour_kernel(const __grid_constant__ KParams p, cons
   const VehC vc = veh_const();
   veh_step_bwd(vc, st, act, lam, abar);          // the state chain runs through done samples too
   if (!frozen) {                                 // reward of step k (masked once done)
-    const float rho = -p.gpow[k] * p.inv_B * (p.reward_shaping ? p.reward_scale : 1.f);
+    const float rho = reward_adjoint(p, k);
     const float r2 = -2.f * p.veh_rscale;
     abar[0] += rho * (r2 * p.veh_rc[5] * act[0]);
     abar[1] += rho * (r2 * p.veh_rc[6] * act[1]);
@@ -275,7 +275,7 @@ __global__ void veh_step_detour_kernel(const __grid_constant__ KParams p, const 
     for (int f = 0; f < obs_dim; ++f) nobs[f] = obs[f];
   }
   if (p.mask_at_done) md = md || dn;
-  if (p.reward_shaping) r = (r + p.reward_shift) * p.reward_scale;
+  r = shape_reward(p, r);
   reward[gs] = r;
   next_done[gs] = md ? 1.f : 0.f;
 }

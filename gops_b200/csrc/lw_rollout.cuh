@@ -7,7 +7,8 @@
 //                     gradient, then the hand-derived adjoint of step k  ->  zbar_k, lambda_k (partial)
 //                     policy MLP backward of slot k (wgmma dgrad GEMMs; deltas kept)  ->  dX_k
 //   weight gradients: ONE contraction per layer over all H x B rows (gops_b200_mlpnet_wgrad_slots).
-// Same per-sample arithmetic as the fused kernels (models.cuh / models_veh.cuh device functions), one thread per sample;
+// The per-sample arithmetic is the fused kernels' own: the wrapper chain, the model steps, the vehicle rewards and their
+// adjoints are the device functions of models.cuh / models_veh.cuh, one thread per sample;
 // states live in HBM between the steps: 0.5 GB of activations per update for C3 (8192 x 60 x [256 + 256 + 248] fp32 x2),
 // 0.1 ms of HBM time -- the path stays tensor / launch bound.
 #pragma once
@@ -88,38 +89,19 @@ __global__ void lw_step_kernel(const __grid_constant__ KParams p, const __grid_c
   float* xn = wx ? a.X + ((size_t)(k + 1) * a.bstride + b) * a.ldx : nullptr;      // the caller allocates H + 1 input slabs
   float r = 0.f;
   if constexpr (M::KIND == 0) {
-    float in[NS];
+    wrapped_step<M>(p, obs_dim, st, act, active, r, dn);
 #pragma unroll
-    for (int f = 0; f < NS; ++f) in[f] = (p.obs_scaling && f < obs_dim) ? st[f] / p.osc[f] - p.osh[f] : st[f];
-    if (active) {
-      bool md = false;
-      const int reps = p.repeat_num > 0 ? p.repeat_num : 1;
-      float rsum = 0.f, rj = 0.f;
-      for (int j = 0; j < reps; ++j) {
-        M::step(p, in, act, rj, md);
-        rsum += rj;
-      }
-      r = (p.repeat_num > 0 && p.sum_reward) ? rsum : rj;
-      dn = md;
-    }
-#pragma unroll
-    for (int f = 0; f < NS; ++f) {
-      float o = (p.obs_scaling && f < obs_dim) ? (in[f] + p.osh[f]) * p.osc[f] : in[f];
-      if (p.clip_obs) o = fminf(fmaxf(o, p.obs_low[f]), p.obs_high[f]);
-      st[f] = o;
-      if (wx && f < obs_dim) xn[f] = o;
-    }
+    for (int f = 0; f < NS; ++f)
+      if (wx && f < obs_dim) xn[f] = st[f];
   } else {
     if (active) {
       const VehC vc = veh_const();
       RefWindow<2, 1> w;
       w.base = p.reference + (size_t)b * p.ref_len * 4;
-      float q[4], o6[6];
+      float q[4];
       w.k0 = p.ref_t + k;
       w.get(0, q);
-      const float ex = st[0] - q[0], ey = st[1] - q[1], ep = angle_normalize(st[2] - q[2]), eu = st[3] - q[3];
-      r = -(0.04f * (ex * ex) + 0.04f * (ey * ey) + 0.02f * (ep * ep) + 0.02f * (eu * eu) + 0.01f * (st[5] * st[5]) +
-            0.01f * (act[0] * act[0]) + 0.01f * (act[1] * act[1]));
+      r = M::reward(st, q, act);
       veh_step(vc, st, act);
       w.k0 = p.ref_t + k + 1;
       if (wx) {      // get_obs of the new state: point i of the window by sub-thread i mod SUB
@@ -130,17 +112,15 @@ __global__ void lw_step_kernel(const __grid_constant__ KParams p, const __grid_c
           ego_obs(st, cs, sn, q[0], q[1], q[2], q[3], o4);
           const int f0 = i == 0 ? 0 : 6 + 4 * (i - 1);
 #pragma unroll
-          for (int c = 0; c < 4; ++c) xn[f0 + c] = p.obs_scaling ? (o4[c] + p.osh[f0 + c]) * p.osc[f0 + c] : o4[c];
+          for (int c = 0; c < 4; ++c) xn[f0 + c] = to_outer(p, f0 + c, o4[c]);
           if (i == 0) {
-            xn[4] = p.obs_scaling ? (st[4] + p.osh[4]) * p.osc[4] : st[4];
-            xn[5] = p.obs_scaling ? (st[5] + p.osh[5]) * p.osc[5] : st[5];
+            xn[4] = to_outer(p, 4, st[4]);
+            xn[5] = to_outer(p, 5, st[5]);
           }
         }
-        (void)o6;
       }
       w.get(0, q);
-      dn = (fabsf(st[0] - q[0]) > 5.f) || (fabsf(st[1] - q[1]) > 2.f) ||
-           (fabsf(angle_normalize(st[2] - q[2])) > 3.14159265358979323846f);
+      dn = M::done(st, q);
     } else if (wx) {
       for (int f = sub; f < obs_dim; f += SUB) xn[f] = xk[f];        // MaskAtDone: the observation is frozen
     }
@@ -150,7 +130,7 @@ __global__ void lw_step_kernel(const __grid_constant__ KParams p, const __grid_c
     if (p.pol.time_input) xn[obs_dim] = (float)(k + 2);
     for (int f = obs_dim + p.pol.time_input; f < a.ldx; ++f) xn[f] = 0.f;
   }
-  if (p.reward_shaping) r = (r + p.reward_shift) * p.reward_scale;
+  r = shape_reward(p, r);
   a.vacc[b] += r * p.gpow[k];
 #pragma unroll
   for (int f = 0; f < NS; ++f) Sn[(size_t)f * B + b] = st[f];
@@ -202,64 +182,20 @@ __global__ void lw_reverse_kernel(const __grid_constant__ KParams p, const __gri
 #pragma unroll
     for (int j = 0; j < MAXA; ++j) z[j] = j < a.act_dim ? a.Z[(size_t)k * a.zs_k + (size_t)b * a.zs_b + j] : 0.f;
     process_action(p, a.act_dim, z, act, g, nullptr);
-    const float rho = -p.gpow[k] * p.inv_B * (p.reward_shaping ? p.reward_scale : 1.f);
+    const float rho = reward_adjoint(p, k);
 #pragma unroll
     for (int j = 0; j < MAXA; ++j) abar[j] = 0.f;
     if constexpr (M::KIND == 0) {
-      const int reps = p.repeat_num > 0 ? p.repeat_num : 1;
-      float in0[NS], cur[NS];
-#pragma unroll
-      for (int f = 0; f < NS; ++f) in0[f] = (p.obs_scaling && f < obs_dim) ? st[f] / p.osc[f] - p.osh[f] : st[f];
-      if (p.clip_obs) {
-        float rr;
-        bool md;
-#pragma unroll
-        for (int f = 0; f < NS; ++f) cur[f] = in0[f];
-        for (int j = 0; j < reps; ++j) M::step(p, cur, act, rr, md);
-#pragma unroll
-        for (int f = 0; f < NS; ++f) {
-          const float o = (p.obs_scaling && f < obs_dim) ? (cur[f] + p.osh[f]) * p.osc[f] : cur[f];
-          if (o < p.obs_low[f] || o > p.obs_high[f]) lam[f] = 0.f;
-        }
-      }
-      if (p.obs_scaling) {
-#pragma unroll
-        for (int f = 0; f < NS; ++f)
-          if (f < obs_dim) lam[f] *= p.osc[f];
-      }
-      for (int j = reps - 1; j >= 0; --j) {
-        float rr, aj[MAXA];
-        bool md;
-#pragma unroll
-        for (int f = 0; f < NS; ++f) cur[f] = in0[f];
-        for (int q = 0; q < j; ++q) M::step(p, cur, act, rr, md);
-        const float rho_j = (p.repeat_num == 0 || p.sum_reward || j == reps - 1) ? rho : 0.f;
-#pragma unroll
-        for (int q = 0; q < MAXA; ++q) aj[q] = 0.f;
-        M::step_bwd(p, cur, act, rho_j, lam, aj);
-#pragma unroll
-        for (int q = 0; q < MAXA; ++q) abar[q] += aj[q];
-      }
-      if (p.obs_scaling) {
-#pragma unroll
-        for (int f = 0; f < NS; ++f)
-          if (f < obs_dim) lam[f] /= p.osc[f];
-      }
+      wrapped_step_bwd<M>(p, obs_dim, st, act, rho, lam, abar);
     } else {
       const VehC vc = veh_const();
       veh_step_bwd(vc, st, act, lam, abar);
-      abar[0] += rho * (-0.02f * act[0]);
-      abar[1] += rho * (-0.02f * act[1]);
       RefWindow<2, 1> w;
       w.base = p.reference + (size_t)b * p.ref_len * 4;
       w.k0 = p.ref_t + k;
       float q[4];
       w.get(0, q);
-      lam[0] += rho * (-0.08f * (st[0] - q[0]));
-      lam[1] += rho * (-0.08f * (st[1] - q[1]));
-      lam[2] += rho * (-0.04f * angle_normalize(st[2] - q[2]));
-      lam[3] += rho * (-0.04f * (st[3] - q[3]));
-      lam[5] += rho * (-0.02f * st[5]);
+      M::reward_bwd(st, q, act, rho, lam, abar);
     }
 #pragma unroll
     for (int j = 0; j < MAXA; ++j) zb[j] = abar[j] * g[j];

@@ -46,6 +46,102 @@ __device__ __forceinline__ void process_action(const KParams& p, int na, const f
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Observation / reward wrappers around the model step (create_env_model.py:104-126), shared by every kernel.
+//   wrapper/scale_observation.py    outer obs = (inner obs + shift) * scale
+//   wrapper/shaping_reward.py       r = (r + shift) * scale, also for masked (done) samples
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ float to_inner(const KParams& p, int f, float x) {
+  return p.obs_scaling ? x / p.osc[f] - p.osh[f] : x;
+}
+__device__ __forceinline__ float to_outer(const KParams& p, int f, float x) {
+  return p.obs_scaling ? (x + p.osh[f]) * p.osc[f] : x;
+}
+__device__ __forceinline__ float shape_reward(const KParams& p, float r) {
+  return p.reward_shaping ? (r + p.reward_shift) * p.reward_scale : r;
+}
+// dL/d(raw reward of step k) of the mean discounted return
+__device__ __forceinline__ float reward_adjoint(const KParams& p, int k) {
+  return -p.gpow[k] * p.inv_B * (p.reward_shaping ? p.reward_scale : 1.f);
+}
+
+// One step of a state==obs model (KIND 0) inside its wrappers, on the outer observation st[0..obs_dim) (in place):
+// ScaleObservation -> ActionRepeat (the masked model step repeated with the same action) -> unscale -> ClipObservation.
+// When `active` (not frozen by MaskAtDone) r receives the raw reward and dn the new done flag; else both are left alone.
+template <class M>
+__device__ __forceinline__ void wrapped_step(const KParams& p, int obs_dim, float* st, const float* a, bool active,
+                                             float& r, bool& dn) {
+  constexpr int NS = M::NS;
+  float in[NS];
+#pragma unroll
+  for (int f = 0; f < NS; ++f) in[f] = (p.obs_scaling && f < obs_dim) ? st[f] / p.osc[f] - p.osh[f] : st[f];
+  if (active) {
+    bool md = false;
+    const int reps = p.repeat_num > 0 ? p.repeat_num : 1;
+    float rsum = 0.f, rj = 0.f;
+    for (int j = 0; j < reps; ++j) {
+      M::step(p, in, a, rj, md);
+      rsum += rj;
+    }
+    r = (p.repeat_num > 0 && p.sum_reward) ? rsum : rj;
+    dn = md;
+  }
+#pragma unroll
+  for (int f = 0; f < NS; ++f) {
+    float o = (p.obs_scaling && f < obs_dim) ? (in[f] + p.osh[f]) * p.osc[f] : in[f];
+    if (p.clip_obs) o = fminf(fmaxf(o, p.obs_low[f]), p.obs_high[f]);
+    st[f] = o;
+  }
+}
+
+// Adjoint of wrapped_step for an active sample: st = outer observation before the step, lam = adjoint of the outer
+// observation after it (in) / before it (out), rho = dL/d(raw reward), abar[j] += dL/d a[j].  Chain of the step:
+//   obs_k -(1/scale, -shift)-> inner_0 -[model step x reps, same action]-> inner_reps -(+shift, *scale)-> clip -> obs_k+1
+template <class M>
+__device__ __forceinline__ void wrapped_step_bwd(const KParams& p, int obs_dim, const float* st, const float* a,
+                                                 float rho, float* lam, float* abar) {
+  constexpr int NS = M::NS;
+  const int reps = p.repeat_num > 0 ? p.repeat_num : 1;
+  float in0[NS], cur[NS];
+#pragma unroll
+  for (int f = 0; f < NS; ++f) in0[f] = (p.obs_scaling && f < obs_dim) ? st[f] / p.osc[f] - p.osh[f] : st[f];
+  if (p.clip_obs) {            // clip passes gradient only where the raw next observation is inside
+    float rr;
+    bool md;
+#pragma unroll
+    for (int f = 0; f < NS; ++f) cur[f] = in0[f];
+    for (int j = 0; j < reps; ++j) M::step(p, cur, a, rr, md);
+#pragma unroll
+    for (int f = 0; f < NS; ++f) {
+      const float o = (p.obs_scaling && f < obs_dim) ? (cur[f] + p.osh[f]) * p.osc[f] : cur[f];
+      if (o < p.obs_low[f] || o > p.obs_high[f]) lam[f] = 0.f;
+    }
+  }
+  if (p.obs_scaling) {
+#pragma unroll
+    for (int f = 0; f < NS; ++f)
+      if (f < obs_dim) lam[f] *= p.osc[f];
+  }
+  for (int j = reps - 1; j >= 0; --j) {
+    float rr, aj[MAXA];
+    bool md;
+#pragma unroll
+    for (int f = 0; f < NS; ++f) cur[f] = in0[f];
+    for (int q = 0; q < j; ++q) M::step(p, cur, a, rr, md);      // state before repeat j
+    const float rho_j = (p.repeat_num == 0 || p.sum_reward || j == reps - 1) ? rho : 0.f;
+#pragma unroll
+    for (int q = 0; q < MAXA; ++q) aj[q] = 0.f;
+    M::step_bwd(p, cur, a, rho_j, lam, aj);
+#pragma unroll
+    for (int q = 0; q < MAXA; ++q) abar[q] += aj[q];
+  }
+  if (p.obs_scaling) {
+#pragma unroll
+    for (int f = 0; f < NS; ++f)
+      if (f < obs_dim) lam[f] /= p.osc[f];
+  }
+}
+
 // =============================================================================================
 // pyth_idpendulum   (env_ocp/env_model/pyth_idpendulum_model.py)
 // state s = [p, th1, th2, pdot, th1dot, th2dot]; 5 explicit-Euler sub-steps of tau = dt/5 with
@@ -242,9 +338,48 @@ struct ModelLq {
 // =============================================================================================
 struct ModelVehConti {
   static constexpr int NS = 7, KIND = 1;   // x, y, phi, u, v, w, ref_time
+  // reward from the INCOMING inner observation o (Veh3dofcontiModel.compute_reward :161-177)
+  __device__ static __forceinline__ float reward(const float* o, const float* a) {
+    return -(0.04f * (o[0] * o[0]) + 0.04f * (o[1] * o[1]) + 0.02f * (o[2] * o[2]) + 0.02f * (o[3] * o[3]) +
+             0.01f * (o[5] * o[5]) + 0.01f * (a[0] * a[0]) + 0.01f * (a[1] * a[1]));
+  }
+  // termination test on the NEW inner observation o
+  __device__ static __forceinline__ bool done(const float* o) {
+    return (fabsf(o[0]) > 10.f) || (fabsf(o[1]) > 10.f) || (fabsf(o[2]) > 3.14159265358979323846f);
+  }
+  // adjoint of reward(): ob[0..5] = dL/d o (entry 4 untouched), abar += dL/d a; rho = dL/d(reward)
+  __device__ static __forceinline__ void reward_bwd(const float* o, const float* a, float rho, float* ob, float* abar) {
+    abar[0] += rho * (-0.02f * a[0]);
+    abar[1] += rho * (-0.02f * a[1]);
+    ob[0] = rho * (-0.08f * o[0]); ob[1] = rho * (-0.08f * o[1]);
+    ob[2] = rho * (-0.04f * o[2]); ob[3] = rho * (-0.04f * o[3]);
+    ob[5] = rho * (-0.02f * o[5]);
+  }
 };
 struct ModelVehTrack {
   static constexpr int NS = 6, KIND = 2;
+  // reward from the CURRENT state s against reference point q = reference[:, t] (veh3dof_tracking_model.py:59-73)
+  __device__ static __forceinline__ float reward(const float* s, const float* q, const float* a) {
+    const float ex = s[0] - q[0], ey = s[1] - q[1], ep = angle_normalize(s[2] - q[2]), eu = s[3] - q[3];
+    return -(0.04f * (ex * ex) + 0.04f * (ey * ey) + 0.02f * (ep * ep) + 0.02f * (eu * eu) + 0.01f * (s[5] * s[5]) +
+             0.01f * (a[0] * a[0]) + 0.01f * (a[1] * a[1]));
+  }
+  // termination test of the new state s against reference[:, t + 1]
+  __device__ static __forceinline__ bool done(const float* s, const float* q) {
+    return (fabsf(s[0] - q[0]) > 5.f) || (fabsf(s[1] - q[1]) > 2.f) ||
+           (fabsf(angle_normalize(s[2] - q[2])) > 3.14159265358979323846f);
+  }
+  // adjoint of reward(): lam += dL/d s, abar += dL/d a; rho = dL/d(reward)
+  __device__ static __forceinline__ void reward_bwd(const float* s, const float* q, const float* a, float rho, float* lam,
+                                                    float* abar) {
+    abar[0] += rho * (-0.02f * a[0]);
+    abar[1] += rho * (-0.02f * a[1]);
+    lam[0] += rho * (-0.08f * (s[0] - q[0]));
+    lam[1] += rho * (-0.08f * (s[1] - q[1]));
+    lam[2] += rho * (-0.04f * angle_normalize(s[2] - q[2]));
+    lam[3] += rho * (-0.04f * (s[3] - q[3]));
+    lam[5] += rho * (-0.02f * s[5]);
+  }
 };
 
 // Accessor of the (P+1)-point reference window of one sample at horizon step k.

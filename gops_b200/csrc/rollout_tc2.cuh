@@ -567,27 +567,8 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           const bool active = valid && (p.mask_at_done ? !dn : true);
           float r = 0.f;
           if (valid) {
-            float in[NS];
-#pragma unroll
-            for (int f = 0; f < NS; ++f) in[f] = (p.obs_scaling && f < obs_dim) ? st[f] / p.osc[f] - p.osh[f] : st[f];
-            if (active) {
-              bool md = false;
-              const int reps = p.repeat_num > 0 ? p.repeat_num : 1;
-              float rsum = 0.f, rj = 0.f;
-              for (int j = 0; j < reps; ++j) {
-                M::step(p, in, a, rj, md);
-                rsum += rj;
-              }
-              r = (p.repeat_num > 0 && p.sum_reward) ? rsum : rj;
-              dn = md;
-            }
-#pragma unroll
-            for (int f = 0; f < NS; ++f) {
-              float o = (p.obs_scaling && f < obs_dim) ? (in[f] + p.osh[f]) * p.osc[f] : in[f];
-              if (p.clip_obs) o = fminf(fmaxf(o, p.obs_low[f]), p.obs_high[f]);
-              st[f] = o;
-            }
-            if (p.reward_shaping) r = (r + p.reward_shift) * p.reward_scale;
+            wrapped_step<M>(p, obs_dim, st, a, active, r, dn);
+            r = shape_reward(p, r);
             vacc += r * p.gpow[k];
           }
           if (alg == ALG_TRACE && valid) {
@@ -709,51 +690,9 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
         if (active) {
           float a[MAXA], g[MAXA], abar[MAXA];
           process_action(p, P.out, zt, a, g, nullptr);
-          const float rho = -p.gpow[k] * p.inv_B * (p.reward_shaping ? p.reward_scale : 1.f);
 #pragma unroll
           for (int j = 0; j < MAXA; ++j) abar[j] = 0.f;
-          // lam = adjoint of the OUTER observation obs_{k+1}.  Chain of step k:
-          //   obs_k -(1/scale, -shift)-> inner_0 -[model step x reps, same action]-> inner_reps
-          //         -(+shift, *scale)-> clip -> obs_{k+1}
-          const int reps = p.repeat_num > 0 ? p.repeat_num : 1;
-          float in0[NS], cur[NS];
-#pragma unroll
-          for (int f = 0; f < NS; ++f) in0[f] = (p.obs_scaling && f < obs_dim) ? st[f] / p.osc[f] - p.osh[f] : st[f];
-          if (p.clip_obs) {            // clip passes gradient only where the raw next observation is inside
-            float rr;
-            bool md;
-#pragma unroll
-            for (int f = 0; f < NS; ++f) cur[f] = in0[f];
-            for (int j = 0; j < reps; ++j) M::step(p, cur, a, rr, md);
-#pragma unroll
-            for (int f = 0; f < NS; ++f) {
-              const float o = (p.obs_scaling && f < obs_dim) ? (cur[f] + p.osh[f]) * p.osc[f] : cur[f];
-              if (o < p.obs_low[f] || o > p.obs_high[f]) lam[f] = 0.f;
-            }
-          }
-          if (p.obs_scaling) {
-#pragma unroll
-            for (int f = 0; f < NS; ++f)
-              if (f < obs_dim) lam[f] *= p.osc[f];
-          }
-          for (int j = reps - 1; j >= 0; --j) {
-            float rr, aj[MAXA];
-            bool md;
-#pragma unroll
-            for (int f = 0; f < NS; ++f) cur[f] = in0[f];
-            for (int q = 0; q < j; ++q) M::step(p, cur, a, rr, md);      // state before repeat j
-            const float rho_j = (p.repeat_num == 0 || p.sum_reward || j == reps - 1) ? rho : 0.f;
-#pragma unroll
-            for (int q = 0; q < MAXA; ++q) aj[q] = 0.f;
-            M::step_bwd(p, cur, a, rho_j, lam, aj);
-#pragma unroll
-            for (int q = 0; q < MAXA; ++q) abar[q] += aj[q];
-          }
-          if (p.obs_scaling) {
-#pragma unroll
-            for (int f = 0; f < NS; ++f)
-              if (f < obs_dim) lam[f] /= p.osc[f];
-          }
+          wrapped_step_bwd<M>(p, obs_dim, st, a, reward_adjoint(p, k), lam, abar);   // lam: adjoint of obs_{k+1}
 #pragma unroll
           for (int j = 0; j < MAXA; ++j) zb[j] = abar[j] * g[j];
         }

@@ -26,16 +26,17 @@ def test_tcf_golden_loss_grad_update(name):
     base.test_golden_loss_grad_update(name)
 
 
-@pytest.mark.parametrize("env_id,algname,act,B,H", [
+@pytest.mark.parametrize("env_id,algname,act,B,H,wk", base.oracle_cases([
     ("pyth_idpendulum", "FHADP", "gelu", 3000, 30),
     ("pyth_idpendulum", "FHADP", "tanh", 777, 7),
     ("pyth_idpendulum", "INFADP", "elu", 2048, 10),
     ("pyth_lq", "INFADP", "gelu", 5000, 10),
     ("pyth_lq", "FHADP", "selu", 1000, 25),
     ("pyth_lq", "INFADP", "sigmoid", 130, 3),
-])
-def test_tcf_against_oracle_fp64(env_id, algname, act, B, H):
-    base.test_against_oracle_fp64(env_id, algname, act, B, H)
+    ("pyth_idpendulum", "FHADP", "gelu", 1500, 10, "obs-rep3last-clip"),
+]))
+def test_tcf_against_oracle_fp64(env_id, algname, act, B, H, wk):
+    base.test_against_oracle_fp64(env_id, algname, act, B, H, wk)
 
 
 @pytest.mark.parametrize("B,H", [(1, 1), (1, 5), (17, 1), (129, 2), (513, 3)])
