@@ -321,7 +321,9 @@ int launch_fused(gops_b200_plan* pl, KParams p, Route route, cudaStream_t st, fl
   long long slots = pl->sm_count;  // CTAs resident at once
   if (tc) {
     const int hact = (alg == ALG_FHADP || pl->pol_tcf.hact == pl->val_tcf.hact) ? pl->pol_tcf.hact : -1;
-    fn = K.tc[hact == GOPS_ACT_GELU][alg];
+    // the fixed-chain kernel, where the model has one, is built for nets with one output (val_tcf = pol_tcf on FHADP)
+    const bool chain = K.tc[kTcGeluChain][alg] && wrap_bits(p) == kTcChain && pl->pol_tcf.out == 1 && pl->val_tcf.out == 1;
+    fn = K.tc[hact != GOPS_ACT_GELU ? kTcGeneric : chain ? kTcGeluChain : kTcGelu][alg];
     if (!fn) return fail("wgmma rollout kernel not built for this env model");
     p.pol = pl->pol_tcf;
     p.val = pl->val_tcf;

@@ -18,13 +18,20 @@ struct LwKernels {      // layer-wise path of the wide nets (lw_rollout.cuh)
 
 struct ModelKernels {
   RolloutFn mma[2][3][4];   // fused mma.sync rollout [hidden 64 / 256][config (hidden 256: 0 only)][alg]
-  RolloutFn tc[2][4];       // fused wgmma rollout [hidden activation at run time / GELU at compile time][alg]
+  RolloutFn tc[3][4];       // fused wgmma rollout [TcVariant][alg]; kTcGeluChain: FHADP only, one output
   LwKernels lw;
   StepFn step;              // gops_b200_model_step of the state == obs models
 };
 
 // families of a model beyond the fused mma.sync rollout
 enum : unsigned { kWgmmaRollout = 1, kModelStep = 2 };
+
+// Instantiations of the wgmma rollout: hidden activation and wrapper flags read at run time; GELU fixed at compile time;
+// GELU, one action and the wrapper chain kTcChain fixed at compile time (FHADP of the models with one action only).
+// kTcChain is what create_env_model builds by default on a model with unbounded observations (idpendulum): ScaleAction
+// + ClipAction, no ScaleObservation, no ActionRepeat, no effective ClipObservation.
+enum TcVariant { kTcGeneric = 0, kTcGelu = 1, kTcGeluChain = 2 };
+constexpr unsigned kTcChain = kWrapActionScale | kWrapClipAction;
 
 static_assert(ALG_FHADP == 0 && ALG_PIM == 1 && ALG_PEV == 2 && ALG_TRACE == 3, "table index = alg");
 
@@ -36,17 +43,21 @@ void set_mma(RolloutFn (&fn)[4]) {
   fn[ALG_TRACE] = rollout_kernel<M, HD, S, NT, ALG_TRACE>;
 }
 
-template <class M, int... AF>   // AF: the activation fixed at compile time (rollout_tc2.cuh, GOPS_TC2_ACT_SWITCH)
+template <class M, int AF, int NA, class W>   // AF, NA, W: see rollout_tc2_kernel
 void set_tc(RolloutFn (&fn)[4]) {
-  fn[ALG_FHADP] = rollout_tc2_kernel<M, ALG_FHADP, AF...>;
-  fn[ALG_PIM] = rollout_tc2_kernel<M, ALG_PIM, AF...>;
-  fn[ALG_PEV] = rollout_tc2_kernel<M, ALG_PEV, AF...>;
-  fn[ALG_TRACE] = rollout_tc2_kernel<M, ALG_TRACE, AF...>;
+  fn[ALG_FHADP] = rollout_tc2_kernel<M, ALG_FHADP, AF, NA, W>;
+  fn[ALG_PIM] = rollout_tc2_kernel<M, ALG_PIM, AF, NA, W>;
+  fn[ALG_PEV] = rollout_tc2_kernel<M, ALG_PEV, AF, NA, W>;
+  fn[ALG_TRACE] = rollout_tc2_kernel<M, ALG_TRACE, AF, NA, W>;
 }
 
 // The layer-wise kernels are passed in by the models that have them, so that lw_rollout.cuh (and its kernels) is only
-// compiled into their objects.
-template <class M, unsigned FAMILIES>
+// compiled into their objects.  NA: 1 for a model with one action, else MAXA.  Only with NA = 1 is the kTcGeluChain
+// FHADP rollout built, for nets with one output.  With MAXA outputs or with the wrapper flags read at run time, fixing
+// NA makes ptxas spill more than the generic kernel does (CUDA 12.9), so those stay generic.  The INFADP kernels stay
+// generic as well: built this way, their value-net weight gradient on idpendulum differs from the generic kernel's in
+// the last bit of a few entries, which the FHADP kernel's results do not.
+template <class M, unsigned FAMILIES, int NA = MAXA>
 ModelKernels model_kernels(LwKernels lw = {}) {
   ModelKernels k = {};
   set_mma<M, 64, 128, 512>(k.mma[0][0]);   // kConfigs of gops_b200.cu: sub-tile S, threads
@@ -54,8 +65,9 @@ ModelKernels model_kernels(LwKernels lw = {}) {
   set_mma<M, 64, 32, 128>(k.mma[0][2]);
   set_mma<M, 256, 32, 256>(k.mma[1][0]);   // kWideConfig
   if constexpr ((FAMILIES & kWgmmaRollout) != 0) {
-    set_tc<M>(k.tc[0]);
-    set_tc<M, GOPS_ACT_GELU>(k.tc[1]);
+    set_tc<M, -1, MAXA, WrapRt>(k.tc[kTcGeneric]);
+    set_tc<M, GOPS_ACT_GELU, MAXA, WrapRt>(k.tc[kTcGelu]);
+    if constexpr (NA == 1) k.tc[kTcGeluChain][ALG_FHADP] = rollout_tc2_kernel<M, ALG_FHADP, GOPS_ACT_GELU, NA, WrapFixed<kTcChain>>;
   }
   if constexpr ((FAMILIES & kModelStep) != 0) k.step = model_step_kernel<M>;
   k.lw = lw;

@@ -6,6 +6,35 @@
 namespace gops {
 
 // ---------------------------------------------------------------------------------------------
+// Flags of the wrapper chain.  WrapRt reads them from KParams at run time; WrapFixed<F> fixes them at compile time
+// (F: kWrap* bits), so that a kernel built for one chain drops the branches of the others.  A fixed chain with
+// kWrapRepeat still reads its repeat count at run time.
+// ---------------------------------------------------------------------------------------------
+enum : unsigned { kWrapObsScaling = 1, kWrapClipObs = 2, kWrapActionScale = 4, kWrapClipAction = 8, kWrapRepeat = 16 };
+
+__host__ __device__ inline unsigned wrap_bits(const KParams& p) {
+  return (p.obs_scaling ? kWrapObsScaling : 0u) | (p.clip_obs ? kWrapClipObs : 0u) |
+         (p.action_scale ? kWrapActionScale : 0u) | (p.clip_action ? kWrapClipAction : 0u) |
+         (p.repeat_num > 0 ? kWrapRepeat : 0u);
+}
+
+struct WrapRt {
+  __device__ static __forceinline__ int obs_scaling(const KParams& p) { return p.obs_scaling; }
+  __device__ static __forceinline__ int clip_obs(const KParams& p) { return p.clip_obs; }
+  __device__ static __forceinline__ int action_scale(const KParams& p) { return p.action_scale; }
+  __device__ static __forceinline__ int clip_action(const KParams& p) { return p.clip_action; }
+  __device__ static __forceinline__ int repeat_num(const KParams& p) { return p.repeat_num; }
+};
+template <unsigned F>
+struct WrapFixed {
+  __device__ static __forceinline__ int obs_scaling(const KParams&) { return (F & kWrapObsScaling) != 0; }
+  __device__ static __forceinline__ int clip_obs(const KParams&) { return (F & kWrapClipObs) != 0; }
+  __device__ static __forceinline__ int action_scale(const KParams&) { return (F & kWrapActionScale) != 0; }
+  __device__ static __forceinline__ int clip_action(const KParams&) { return (F & kWrapClipAction) != 0; }
+  __device__ static __forceinline__ int repeat_num(const KParams& p) { return (F & kWrapRepeat) != 0 ? p.repeat_num : 0; }
+};
+
+// ---------------------------------------------------------------------------------------------
 // Policy output -> model action through tanh squashing + ScaleAction + ClipAction.
 //   mlp.py:73-77 / :103-111          a_pol = (hi-lo)/2 * tanh(z) + (hi+lo)/2
 //   wrapper/scale_action.py:75-83    clip -> affine -> clip
@@ -13,9 +42,10 @@ namespace gops {
 // a[j]: action handed to the model, g[j] = d a[j] / d z[j] (clip gradient = 1 inside, inclusive).
 // ---------------------------------------------------------------------------------------------
 // ScaleAction + ClipAction applied to one policy-output component x; gg is multiplied by d(out)/dx
+template <class W = WrapRt>
 __device__ __forceinline__ float wrap_action(const KParams& p, int j, float x, float& gg) {
   const float lo = p.act_low[j], hi = p.act_high[j];
-  if (p.action_scale) {
+  if (W::action_scale(p)) {
     const float mn = p.min_action[j], mx = p.max_action[j];
     if (x < mn || x > mx) gg = 0.f;
     x = fminf(fmaxf(x, mn), mx);
@@ -25,23 +55,25 @@ __device__ __forceinline__ float wrap_action(const KParams& p, int j, float x, f
     if (x < lo || x > hi) gg = 0.f;
     x = fminf(fmaxf(x, lo), hi);
   }
-  if (p.clip_action) {
+  if (W::clip_action(p)) {
     if (x < lo || x > hi) gg = 0.f;
     x = fminf(fmaxf(x, lo), hi);
   }
   return x;
 }
 
+// NA: length of the arrays (the kernel's action count, >= na)
+template <int NA = MAXA, class W = WrapRt>
 __device__ __forceinline__ void process_action(const KParams& p, int na, const float* z, float* a, float* g,
                                                float* apol_out) {
 #pragma unroll
-  for (int j = 0; j < MAXA; ++j) {
+  for (int j = 0; j < NA; ++j) {
     if (j >= na) { a[j] = 0.f; g[j] = 0.f; if (apol_out) apol_out[j] = 0.f; continue; }
     const float th = tanhf(z[j]);
     const float x = __fadd_rn(__fmul_rn(p.pol_half[j], th), p.pol_mid[j]);
     float gg = p.pol_half[j] * (1.f - th * th);
     if (apol_out) apol_out[j] = x;
-    a[j] = wrap_action(p, j, x, gg);
+    a[j] = wrap_action<W>(p, j, x, gg);
     g[j] = gg;
   }
 }
@@ -68,28 +100,28 @@ __device__ __forceinline__ float reward_adjoint(const KParams& p, int k) {
 // One step of a state==obs model (KIND 0) inside its wrappers, on the outer observation st[0..obs_dim) (in place):
 // ScaleObservation -> ActionRepeat (the masked model step repeated with the same action) -> unscale -> ClipObservation.
 // When `active` (not frozen by MaskAtDone) r receives the raw reward and dn the new done flag; else both are left alone.
-template <class M>
+template <class M, class W = WrapRt>
 __device__ __forceinline__ void wrapped_step(const KParams& p, int obs_dim, float* st, const float* a, bool active,
                                              float& r, bool& dn) {
   constexpr int NS = M::NS;
   float in[NS];
 #pragma unroll
-  for (int f = 0; f < NS; ++f) in[f] = (p.obs_scaling && f < obs_dim) ? st[f] / p.osc[f] - p.osh[f] : st[f];
+  for (int f = 0; f < NS; ++f) in[f] = (W::obs_scaling(p) && f < obs_dim) ? st[f] / p.osc[f] - p.osh[f] : st[f];
   if (active) {
     bool md = false;
-    const int reps = p.repeat_num > 0 ? p.repeat_num : 1;
+    const int reps = W::repeat_num(p) > 0 ? W::repeat_num(p) : 1;
     float rsum = 0.f, rj = 0.f;
     for (int j = 0; j < reps; ++j) {
       M::step(p, in, a, rj, md);
       rsum += rj;
     }
-    r = (p.repeat_num > 0 && p.sum_reward) ? rsum : rj;
+    r = (W::repeat_num(p) > 0 && p.sum_reward) ? rsum : rj;
     dn = md;
   }
 #pragma unroll
   for (int f = 0; f < NS; ++f) {
-    float o = (p.obs_scaling && f < obs_dim) ? (in[f] + p.osh[f]) * p.osc[f] : in[f];
-    if (p.clip_obs) o = fminf(fmaxf(o, p.obs_low[f]), p.obs_high[f]);
+    float o = (W::obs_scaling(p) && f < obs_dim) ? (in[f] + p.osh[f]) * p.osc[f] : in[f];
+    if (W::clip_obs(p)) o = fminf(fmaxf(o, p.obs_low[f]), p.obs_high[f]);
     st[f] = o;
   }
 }
@@ -97,15 +129,16 @@ __device__ __forceinline__ void wrapped_step(const KParams& p, int obs_dim, floa
 // Adjoint of wrapped_step for an active sample: st = outer observation before the step, lam = adjoint of the outer
 // observation after it (in) / before it (out), rho = dL/d(raw reward), abar[j] += dL/d a[j].  Chain of the step:
 //   obs_k -(1/scale, -shift)-> inner_0 -[model step x reps, same action]-> inner_reps -(+shift, *scale)-> clip -> obs_k+1
-template <class M>
+// NA: length of abar (the kernel's action count; M reads a[0, NA) and writes at most MAXA adjoints).
+template <class M, int NA = MAXA, class W = WrapRt>
 __device__ __forceinline__ void wrapped_step_bwd(const KParams& p, int obs_dim, const float* st, const float* a,
                                                  float rho, float* lam, float* abar) {
   constexpr int NS = M::NS;
-  const int reps = p.repeat_num > 0 ? p.repeat_num : 1;
+  const int reps = W::repeat_num(p) > 0 ? W::repeat_num(p) : 1;
   float in0[NS], cur[NS];
 #pragma unroll
-  for (int f = 0; f < NS; ++f) in0[f] = (p.obs_scaling && f < obs_dim) ? st[f] / p.osc[f] - p.osh[f] : st[f];
-  if (p.clip_obs) {            // clip passes gradient only where the raw next observation is inside
+  for (int f = 0; f < NS; ++f) in0[f] = (W::obs_scaling(p) && f < obs_dim) ? st[f] / p.osc[f] - p.osh[f] : st[f];
+  if (W::clip_obs(p)) {            // clip passes gradient only where the raw next observation is inside
     float rr;
     bool md;
 #pragma unroll
@@ -113,11 +146,11 @@ __device__ __forceinline__ void wrapped_step_bwd(const KParams& p, int obs_dim, 
     for (int j = 0; j < reps; ++j) M::step(p, cur, a, rr, md);
 #pragma unroll
     for (int f = 0; f < NS; ++f) {
-      const float o = (p.obs_scaling && f < obs_dim) ? (cur[f] + p.osh[f]) * p.osc[f] : cur[f];
+      const float o = (W::obs_scaling(p) && f < obs_dim) ? (cur[f] + p.osh[f]) * p.osc[f] : cur[f];
       if (o < p.obs_low[f] || o > p.obs_high[f]) lam[f] = 0.f;
     }
   }
-  if (p.obs_scaling) {
+  if (W::obs_scaling(p)) {
 #pragma unroll
     for (int f = 0; f < NS; ++f)
       if (f < obs_dim) lam[f] *= p.osc[f];
@@ -128,14 +161,14 @@ __device__ __forceinline__ void wrapped_step_bwd(const KParams& p, int obs_dim, 
 #pragma unroll
     for (int f = 0; f < NS; ++f) cur[f] = in0[f];
     for (int q = 0; q < j; ++q) M::step(p, cur, a, rr, md);      // state before repeat j
-    const float rho_j = (p.repeat_num == 0 || p.sum_reward || j == reps - 1) ? rho : 0.f;
+    const float rho_j = (W::repeat_num(p) == 0 || p.sum_reward || j == reps - 1) ? rho : 0.f;
 #pragma unroll
     for (int q = 0; q < MAXA; ++q) aj[q] = 0.f;
     M::step_bwd(p, cur, a, rho_j, lam, aj);
 #pragma unroll
-    for (int q = 0; q < MAXA; ++q) abar[q] += aj[q];
+    for (int q = 0; q < NA; ++q) abar[q] += aj[q];
   }
-  if (p.obs_scaling) {
+  if (W::obs_scaling(p)) {
 #pragma unroll
     for (int f = 0; f < NS; ++f)
       if (f < obs_dim) lam[f] /= p.osc[f];

@@ -32,6 +32,7 @@
 #pragma once
 #include "models.cuh"
 #include "mlp_tc_full.cuh"
+#include "tc2_probe.cuh"
 
 namespace gops {
 namespace tc2 {
@@ -245,13 +246,20 @@ __device__ __forceinline__ void layer2_product(const Grp& G, const NetL& L, floa
   wg::wait<0>();
   wg::reg_fence<32>(d);
 }
+// NA: the kernel's action count = length of the per-output arrays (z, zbar, S, Acc3).  Every net has at least one
+// output; with NA = 1 that is all of them (the host selects such a kernel only for nets with one output), so output a
+// is live without a test.
+template <int NA>
+__device__ __forceinline__ bool live(int a, const NetL& L) { return NA == 1 || a < L.out; }
+
 // output layer: S[q][a] = this thread's (even, odd) column sums of W3[a] . h for fragment row q; reduced over the four
 // lanes of the quad, the owner of each row takes z[a] = b3[a] + W3[a] . h
-__device__ __forceinline__ void output_sum(const Grp& G, const NetL& L, f32x2::u64 (*S)[MAXA], float* z) {
+template <int NA>
+__device__ __forceinline__ void output_sum(const Grp& G, const NetL& L, f32x2::u64 (*S)[NA], float* z) {
 #pragma unroll
-  for (int a = 0; a < MAXA; ++a) {
+  for (int a = 0; a < NA; ++a) {
     z[a] = 0.f;
-    if (a < L.out) {
+    if (live<NA>(a, L)) {
       float s[2];
 #pragma unroll
       for (int q = 0; q < 2; ++q) {
@@ -265,22 +273,23 @@ __device__ __forceinline__ void output_sum(const Grp& G, const NetL& L, f32x2::u
     }
   }
 }
+template <int NA>
 __device__ __forceinline__ void output_layer(const Grp& G, const NetL& L, const float* h, float* z) {
-  f32x2::u64 S[2][MAXA];
+  f32x2::u64 S[2][NA];
 #pragma unroll
-  for (int a = 0; a < MAXA; ++a) S[0][a] = S[1][a] = f32x2::rep(0.f);
+  for (int a = 0; a < NA; ++a) S[0][a] = S[1][a] = f32x2::rep(0.f);
 #pragma unroll
   for (int i = 0; i < 32; i += 2) {
     const int col = wg::frag_col(G.t, i), q = (i >> 1) & 1;
 #pragma unroll
-    for (int a = 0; a < MAXA; ++a)
-      if (a < L.out) S[q][a] = f32x2::fma(f32x2::ld(G.W3(L) + a * 64 + col), f32x2::pk(h[i], h[i + 1]), S[q][a]);
+    for (int a = 0; a < NA; ++a)
+      if (live<NA>(a, L)) S[q][a] = f32x2::fma(f32x2::ld(G.W3(L) + a * 64 + col), f32x2::pk(h[i], h[i + 1]), S[q][a]);
   }
-  output_sum(G, L, S, z);
+  output_sum<NA>(G, L, S, z);
 }
 
 // layer 2 + output layer, forward only: the owner gets z[a] = b3[a] + W3[a] . act(H1 . W2^T + b2)
-template <int AF>
+template <int AF, int NA>
 __device__ __forceinline__ void layer2_out(const Grp& G, const NetL& L, float* z) {
   float d[32];
   layer2_product(G, L, d);
@@ -289,23 +298,24 @@ __device__ __forceinline__ void layer2_out(const Grp& G, const NetL& L, float* z
       act_fwd_pair_t<A>(f32x2::add(f32x2::pk(d[i], d[i + 1]), f32x2::ld(G.b2(L) + wg::frag_col(G.t, i))), d[i], d[i + 1]);
   GOPS_TC2_ACT_SWITCH(AF, L.hact, GOPS_TC2_A2)
 #undef GOPS_TC2_A2
-  output_layer(G, L, d, z);
+  output_layer<NA>(G, L, d, z);
 }
 
 // Per-thread accumulators of the output-layer gradients: lane l of warp w holds dW3[a] of columns 8 (l / 4) + 2 (l % 4)
 // + {0, 1}, summed over the warp's 16 rows; the owners hold their rows' db3.  Combined across the warps once, at the end
 // of the kernel.
+template <int NA>
 struct Acc3 {
-  float w[MAXA][2];
-  float b[MAXA];
+  float w[NA][2];
+  float b[NA];
 };
 
 // layer 2 epilogue of the backward pass, one column pair of both fragment rows at a time: h = act(pre2), then
 // delta2 = act'(pre2) * (W3^T zbar) straight into the two delta planes, WANT_DW: the dW3 sums (over the warp's rows by
 // an xor butterfly over the quads), WANT_Z: the output-layer partial sums S (output_layer).  zr: zbar of the two rows.
-template <int A, bool WANT_DW, bool WANT_Z>
-__device__ __forceinline__ void delta2_epilogue(const Grp& G, const NetL& L, float* d, const float (*zr)[MAXA], Acc3& acc3,
-                                                f32x2::u64 (*S)[MAXA]) {
+template <int A, bool WANT_DW, bool WANT_Z, int NA>
+__device__ __forceinline__ void delta2_epilogue(const Grp& G, const NetL& L, float* d, const float (*zr)[NA],
+                                                Acc3<NA>& acc3, f32x2::u64 (*S)[NA]) {
   const int q4 = (G.t & 31) >> 2;
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
@@ -318,8 +328,8 @@ __device__ __forceinline__ void delta2_epilogue(const Grp& G, const NetL& L, flo
       act_fwd_grad_pair_t<A>(f32x2::add(f32x2::pk(d[i], d[i + 1]), f32x2::ld(G.b2(L) + col)), h[q][0], h[q][1], g0, g1);
       f32x2::u64 gs = f32x2::rep(0.f);
 #pragma unroll
-      for (int a = 0; a < MAXA; ++a)
-        if (a < L.out) gs = f32x2::fma(f32x2::ld(G.W3(L) + a * 64 + col), f32x2::rep(zr[q][a]), gs);
+      for (int a = 0; a < NA; ++a)
+        if (live<NA>(a, L)) gs = f32x2::fma(f32x2::ld(G.W3(L) + a * 64 + col), f32x2::rep(zr[q][a]), gs);
       uint32_t w0, w1;
       split2(f32x2::mul(f32x2::pk(g0, g1), gs), w0, w1);
       const int off = j * (GT * 16) + wg::frag_row(G.t, i) * 16 + 4 * G.c;
@@ -327,14 +337,14 @@ __device__ __forceinline__ void delta2_epilogue(const Grp& G, const NetL& L, flo
       *reinterpret_cast<uint32_t*>(G.Q() + HPL + off) = w1;
       if constexpr (WANT_Z) {
 #pragma unroll
-        for (int a = 0; a < MAXA; ++a)
-          if (a < L.out) S[q][a] = f32x2::fma(f32x2::ld(G.W3(L) + a * 64 + col), f32x2::pk(h[q][0], h[q][1]), S[q][a]);
+        for (int a = 0; a < NA; ++a)
+          if (live<NA>(a, L)) S[q][a] = f32x2::fma(f32x2::ld(G.W3(L) + a * 64 + col), f32x2::pk(h[q][0], h[q][1]), S[q][a]);
       }
     }
     if constexpr (WANT_DW) {
 #pragma unroll
-      for (int a = 0; a < MAXA; ++a)
-        if (a < L.out) {
+      for (int a = 0; a < NA; ++a)
+        if (live<NA>(a, L)) {
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             float v = fmaf(zr[1][a], h[1][e], zr[0][a] * h[0][e]);
@@ -350,64 +360,78 @@ __device__ __forceinline__ void delta2_epilogue(const Grp& G, const NetL& L, flo
 
 // layer 2 recompute fused with the start of the backward pass: z for the owner (WANT_Z), dW3 / db3 sums, and
 // delta2 -> the two delta planes.  zbar: the owner's output adjoint of its row.
-template <bool WANT_DW, bool WANT_Z, int AF>
-__device__ __forceinline__ void layer2_back(const Grp& G, const NetL& L, const float* zbar, float* z, Acc3& acc3) {
+template <bool WANT_DW, bool WANT_Z, int AF, int NA>
+__device__ __forceinline__ void layer2_back(const Grp& G, const NetL& L, const float* zbar, float* z, Acc3<NA>& acc3) {
   float d[32];
   layer2_product(G, L, d);
   const int qb = (G.t & 31) & ~3;
-  float zr[2][MAXA];                              // zbar of the fragment's two rows
+  float zr[2][NA];                                // zbar of the fragment's two rows
 #pragma unroll
-  for (int a = 0; a < MAXA; ++a) {
+  for (int a = 0; a < NA; ++a) {
     zr[0][a] = __shfl_sync(0xffffffffu, zbar[a], qb);
     zr[1][a] = __shfl_sync(0xffffffffu, zbar[a], qb + 1);
   }
-  f32x2::u64 S[2][MAXA];
+  f32x2::u64 S[2][NA];
 #pragma unroll
-  for (int a = 0; a < MAXA; ++a) S[0][a] = S[1][a] = f32x2::rep(0.f);
-#define GOPS_TC2_A3(A) delta2_epilogue<A, WANT_DW, WANT_Z>(G, L, d, zr, acc3, S);
+  for (int a = 0; a < NA; ++a) S[0][a] = S[1][a] = f32x2::rep(0.f);
+#define GOPS_TC2_A3(A) delta2_epilogue<A, WANT_DW, WANT_Z, NA>(G, L, d, zr, acc3, S);
   GOPS_TC2_ACT_SWITCH(AF, L.hact, GOPS_TC2_A3)
 #undef GOPS_TC2_A3
-  if constexpr (WANT_Z) output_sum(G, L, S, z);
+  if constexpr (WANT_Z) output_sum<NA>(G, L, S, z);
   if constexpr (WANT_DW) {
 #pragma unroll
-    for (int a = 0; a < MAXA; ++a)
-      if (a < L.out && G.own) acc3.b[a] += zbar[a];
+    for (int a = 0; a < NA; ++a)
+      if (live<NA>(a, L) && G.own) acc3.b[a] += zbar[a];
   }
 }
 
 // delta2 planes -> delta1 = (delta2 . W2) * act'(pre1) (same planes, once the readers of delta2 retired) -> the owner's
 // input gradient dx (want_dx) and, WANT_DW, the weight gradients of both layers added into the partial `part`.
-// x: the observation planes of this step's layer 1.
-template <bool WANT_DW, int NS>
+// x: the observation planes of this step's layer 1.  pr: phase probe (tc2_probe.cuh), stamps the delta2 / dW2 part.
+// OVERLAP (WANT_DW): delta2 . W2 and the layer-2 weight gradients go out as two commit groups of one issue, and delta1
+// is formed while the second runs.  Its 40 accumulators are live across delta1, so only the NA = 1 kernels take it (with
+// MAXA outputs ptxas spills more).
+template <bool WANT_DW, int NS, bool OVERLAP>
 __device__ __forceinline__ void backprop(const Grp& G, const NetL& L, bool want_dx, float* __restrict__ part,
-                                         const unsigned char* x, const float* a1p, float* dx) {
+                                         const unsigned char* x, const float* a1p, float* dx, Probe& pr) {
   using namespace tcf;
   publish(G);                                     // delta2 planes visible
-  float g1[32];
+  // delta2 . W2 and the layer-2 weight gradients read only the delta2 and H1 planes
+  constexpr bool overlap = WANT_DW && OVERLAP;
+  float g1[32], w[32], wb[8];
   wg::fence();
   mma_dw<64, 4>(g1, k_act(G.Q(), HPL), mn_w(G.W2(L), W2PLANE));
   wg::commit();
-  wg::wait<0>();
+  if constexpr (overlap) {
+    mma_wgrad<64, 2>(w, mn_act(G.Q(), HPL), mn_act(G.P, HPL));
+    mma_wgrad<16, 1>(wb, mn_act(G.Q(), HPL), ones_op(G));
+    wg::commit();
+    wg::wait<1>();
+  } else {
+    wg::wait<0>();
+  }
   wg::reg_fence<32>(g1);
   if (!WANT_DW && !want_dx) return;
 #pragma unroll
   for (int i = 0; i < 32; ++i) g1[i] *= a1p[i];   // delta1, written once the wgmma reads of delta2 have retired
   if constexpr (WANT_DW) {
-    float w[32], wb[8];
-    wg::fence();
-    mma_wgrad<64, 2>(w, mn_act(G.Q(), HPL), mn_act(G.P, HPL));
-    mma_wgrad<16, 1>(wb, mn_act(G.Q(), HPL), ones_op(G));
-    wg::commit();
+    if constexpr (!overlap) {
+      wg::fence();
+      mma_wgrad<64, 2>(w, mn_act(G.Q(), HPL), mn_act(G.P, HPL));
+      mma_wgrad<16, 1>(wb, mn_act(G.Q(), HPL), ones_op(G));
+      wg::commit();
+    }
     wg::wait<0>();
     wg::reg_fence<32>(w);
     wg::reg_fence<8>(wb);
     red_frag<64, true>(part + L.g_w2, 64, 64, w, G.t);
     red_bias(part + L.g_b2, wb, G);
   }
+  pr.stamp(kRevD2);
   wg::wg_sync(G.g);                               // every wgmma read of delta2 retired
   frag_to_planes<2>(G.Q(), G, g1);
   publish(G);                                     // delta1 planes visible
-  float d[8], w[8], wb[8];
+  float d[8], w1[8], wb1[8];
   if (want_dx) {
     wg::fence();
     mma_dw<16, 4>(d, k_act(G.Q(), HPL), mn_w(G.W1(L), W1PLANE));
@@ -415,16 +439,16 @@ __device__ __forceinline__ void backprop(const Grp& G, const NetL& L, bool want_
   }
   if constexpr (WANT_DW) {
     wg::fence();
-    mma_wgrad<16, 2>(w, mn_act(G.Q(), HPL), mn_act(x, XPL));
-    mma_wgrad<16, 1>(wb, mn_act(G.Q(), HPL), ones_op(G));
+    mma_wgrad<16, 2>(w1, mn_act(G.Q(), HPL), mn_act(x, XPL));
+    mma_wgrad<16, 1>(wb1, mn_act(G.Q(), HPL), ones_op(G));
     wg::commit();
   }
   wg::wait<0>();
   if constexpr (WANT_DW) {
-    wg::reg_fence<8>(w);
-    wg::reg_fence<8>(wb);
-    red_frag<16, false>(part + L.g_w1, L.in, L.in, w, G.t);
-    red_bias(part + L.g_b1, wb, G);
+    wg::reg_fence<8>(w1);
+    wg::reg_fence<8>(wb1);
+    red_frag<16, false>(part + L.g_w1, L.in, L.in, w1, G.t);
+    red_bias(part + L.g_b1, wb1, G);
   }
   if (want_dx) {
     wg::reg_fence<8>(d);
@@ -452,11 +476,14 @@ __device__ __forceinline__ void backprop(const Grp& G, const NetL& L, bool want_
 // The kernel.  grid = min(#SM, #sub-tiles) CTAs of WGS warpgroups, one CTA per SM (shared memory).
 // Slot s = WGS * blockIdx.x + warpgroup owns the contiguous sub-tile range [NSUB s / slots, NSUB (s + 1) / slots), its
 // tape columns and its row of the gradient partials.
+// AF: hidden activation (GOPS_TC2_ACT_SWITCH).  NA: action count, MAXA (policy outputs read from the plan) or 1 (nets
+// with one output: the per-output arrays and tests drop out).  W: wrapper flags (models.cuh, WrapRt / WrapFixed).
 // ---------------------------------------------------------------------------------------------------------------
-template <class M, int ALG, int AF = -1>
+template <class M, int ALG, int AF, int NA, class W>
 __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_constant__ KParams p) {
   using namespace tc2;
   static_assert(M::KIND == 0, "wgmma rollout kernel: state == obs models");
+  static_assert(NA == 1 || NA == MAXA, "wgmma rollout kernel: NA is MAXA or 1");
   constexpr int NS = M::NS, alg = ALG;
   extern __shared__ __align__(16) float smem[];
   unsigned char* sm = reinterpret_cast<unsigned char*>(smem);
@@ -504,16 +531,19 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
   const NetL& P = p.pol;
   const NetL& V = p.val;
   const int H = p.horizon, obs_dim = P.obs, TCH = p.tape_ch;
+  const int pout = NA == 1 ? 1 : P.out;                        // policy outputs
   const long long B = p.batch;
   const int slot = blockIdx.x * WGS + G.g, slots = gridDim.x * WGS;
   // zeroed before the first red.global.add into it: stage() below is a CTA barrier
   float* part = p.partial + (size_t)slot * p.part_stride;
   for (int i = G.t; i < p.part_stride; i += 128) part[i] = 0.f;
   float* tape = p.tape + (size_t)slot * (size_t)H * TCH * GT;
-  Acc3 acc3;
+  Acc3<NA> acc3;
 #pragma unroll
-  for (int a = 0; a < MAXA; ++a) acc3.w[a][0] = acc3.w[a][1] = acc3.b[a] = 0.f;
+  for (int a = 0; a < NA; ++a) acc3.w[a][0] = acc3.w[a][1] = acc3.b[a] = 0.f;
   float loss_acc = 0.f, vmean_acc = 0.f, done_acc = 0.f;
+  Probe pr;
+  pr.init(G.t);
 
   for (int i = G.t; i < 2 * XP_BYTES / 16; i += 128) reinterpret_cast<uint4*>(G.X(0))[i] = make_uint4(0u, 0u, 0u, 0u);
   stage(p.blob_pol, P.blob);      // (its leading CTA barrier also publishes the zeroed planes)
@@ -544,6 +574,7 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
     // ================================ forward sweep ================================
     if (have) {
       for (int k = 0; k < H; ++k) {
+        pr.mark();
         if (own) {
           if (alg == ALG_FHADP || alg == ALG_PIM) {
 #pragma unroll
@@ -551,23 +582,25 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
             tape[(k * TCH + NS) * GT + G.row] = dn ? 1.f : 0.f;
           }
         }
-        float z[MAXA], d1[32];
+        float z[NA], d1[32];
         put_x<NS>(G, G.X(k), P, st, (float)(k + 1));
         layer1_issue(G, P, G.X(k), d1);
         layer1_finish<false, AF>(G, P, d1, nullptr);
-        layer2_out<AF>(G, P, z);
+        pr.stamp(kFwdL1);
+        layer2_out<AF, NA>(G, P, z);
+        pr.stamp(kFwdL2);
         if (own) {
-          float a[MAXA], g[MAXA], apol[MAXA];
+          float a[NA], g[NA], apol[NA];
           if (alg == ALG_FHADP || alg == ALG_PIM) {
 #pragma unroll
-            for (int j = 0; j < MAXA; ++j)
-              if (j < P.out) tape[(k * TCH + NS + 1 + j) * GT + G.row] = z[j];
+            for (int j = 0; j < NA; ++j)
+              if (j < pout) tape[(k * TCH + NS + 1 + j) * GT + G.row] = z[j];
           }
-          process_action(p, P.out, z, a, g, apol);
+          process_action<NA, W>(p, pout, z, a, g, apol);
           const bool active = valid && (p.mask_at_done ? !dn : true);
           float r = 0.f;
           if (valid) {
-            wrapped_step<M>(p, obs_dim, st, a, active, r, dn);
+            wrapped_step<M, W>(p, obs_dim, st, a, active, r, dn);
             r = shape_reward(p, r);
             vacc += r * p.gpow[k];
           }
@@ -576,11 +609,13 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
             if (p.tr_obs)
               for (int f = 0; f < obs_dim; ++f) p.tr_obs[row * obs_dim + f] = st[f];
             if (p.tr_act)
-              for (int j = 0; j < P.out; ++j) p.tr_act[row * P.out + j] = apol[j];
+              for (int j = 0; j < pout; ++j) p.tr_act[row * pout + j] = apol[j];
             if (p.tr_rew) p.tr_rew[row] = r;
             if (p.tr_done) p.tr_done[row] = dn ? 1.f : 0.f;
           }
         }
+        pr.stamp(kFwdDyn);
+        pr.step(true);
       }
       if (valid && dn) done_acc += 1.f;
     }
@@ -595,17 +630,17 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
       if (have) {
         const float gn = p.gpow[H];
         const bool term = valid && !dn;
-        float zv[MAXA], zb[MAXA], d1[32], a1p[32];
+        float zv[NA], zb[NA], d1[32], a1p[32];
 #pragma unroll
-        for (int j = 0; j < MAXA; ++j) zb[j] = zv[j] = 0.f;
+        for (int j = 0; j < NA; ++j) zb[j] = zv[j] = 0.f;
         put_x<NS>(G, G.X(0), V, st, 0.f);
         layer1_issue(G, V, G.X(0), d1);
         if (alg == ALG_PIM) {
           float dx[NS];
           zb[0] = term ? -gn * p.inv_B : 0.f;
           layer1_finish<true, AF>(G, V, d1, a1p);
-          layer2_back<false, true, AF>(G, V, zb, zv, acc3);
-          backprop<false, NS>(G, V, true, part, G.X(0), a1p, dx);
+          layer2_back<false, true, AF, NA>(G, V, zb, zv, acc3);
+          backprop<false, NS, NA == 1>(G, V, true, part, G.X(0), a1p, dx, pr);
           if (term) {
 #pragma unroll
             for (int f = 0; f < NS; ++f)
@@ -613,7 +648,7 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           }
         } else {
           layer1_finish<false, AF>(G, V, d1, nullptr);
-          layer2_out<AF>(G, V, zv);
+          layer2_out<AF, NA>(G, V, zv);
         }
         if (term) vacc += gn * zv[0];
       }
@@ -626,22 +661,22 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
         float o0[NS];
 #pragma unroll
         for (int f = 0; f < NS; ++f) o0[f] = (valid && f < obs_dim) ? p.obs[gs * obs_dim + f] : 0.f;
-        float zv[MAXA], zb[MAXA], d1[32], a1p[32];
+        float zv[NA], zb[NA], d1[32], a1p[32];
 #pragma unroll
-        for (int j = 0; j < MAXA; ++j) zb[j] = zv[j] = 0.f;
+        for (int j = 0; j < NA; ++j) zb[j] = zv[j] = 0.f;
         // the output adjoint needs v(o_0) first: forward to the output, then recompute layer 2 fused with the backward
         put_x<NS>(G, G.X(0), V, o0, 0.f);
         layer1_issue(G, V, G.X(0), d1);
         layer1_finish<true, AF>(G, V, d1, a1p);
-        layer2_out<AF>(G, V, zv);
+        layer2_out<AF, NA>(G, V, zv);
         if (valid) {
           const float diff = zv[0] - vacc;
           loss_acc += diff * diff * p.inv_B;
           vmean_acc += zv[0] * p.inv_B;
           zb[0] = 2.f * diff * p.inv_B;
         }
-        layer2_back<true, false, AF>(G, V, zb, nullptr, acc3);
-        backprop<true, NS>(G, V, false, part, G.X(0), a1p, nullptr);
+        layer2_back<true, false, AF, NA>(G, V, zb, nullptr, acc3);
+        backprop<true, NS, NA == 1>(G, V, false, part, G.X(0), a1p, nullptr, pr);
       }
       stage(p.blob_pol, P.blob);
       continue;
@@ -663,23 +698,25 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
       ndn = tape[((H - 1) * TCH + NS) * GT + G.row] != 0.f;
     }
     for (int k = H - 1; k >= 0; --k) {
-      float zt[MAXA];
+      pr.mark();
+      float zt[NA];
       const bool dnk = ndn;
 #pragma unroll
       for (int f = 0; f < NS; ++f) st[f] = nst[f];
 #pragma unroll
-      for (int j = 0; j < MAXA; ++j) zt[j] = 0.f;
+      for (int j = 0; j < NA; ++j) zt[j] = 0.f;
       if (own) {
 #pragma unroll
-        for (int j = 0; j < MAXA; ++j)
-          if (j < P.out) zt[j] = tape[(k * TCH + NS + 1 + j) * GT + G.row];
+        for (int j = 0; j < NA; ++j)
+          if (j < pout) zt[j] = tape[(k * TCH + NS + 1 + j) * GT + G.row];
       }
       float d1[32], a1p[32];
       put_x<NS>(G, G.X(k), P, st, (float)(k + 1));
       layer1_issue(G, P, G.X(k), d1);                // recompute of step k's layer 1, overlapped with the adjoint
-      float zb[MAXA];
+      pr.stamp(kRevL1);
+      float zb[NA];
 #pragma unroll
-      for (int j = 0; j < MAXA; ++j) zb[j] = 0.f;
+      for (int j = 0; j < NA; ++j) zb[j] = 0.f;
       const bool active = valid && (p.mask_at_done ? !dnk : true);
       if (own) {
         if (k > 0) {
@@ -688,24 +725,29 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           ndn = tape[((k - 1) * TCH + NS) * GT + G.row] != 0.f;
         }
         if (active) {
-          float a[MAXA], g[MAXA], abar[MAXA];
-          process_action(p, P.out, zt, a, g, nullptr);
+          float a[NA], g[NA], abar[NA];
+          process_action<NA, W>(p, pout, zt, a, g, nullptr);
 #pragma unroll
-          for (int j = 0; j < MAXA; ++j) abar[j] = 0.f;
-          wrapped_step_bwd<M>(p, obs_dim, st, a, reward_adjoint(p, k), lam, abar);   // lam: adjoint of obs_{k+1}
+          for (int j = 0; j < NA; ++j) abar[j] = 0.f;
+          wrapped_step_bwd<M, NA, W>(p, obs_dim, st, a, reward_adjoint(p, k), lam, abar);   // lam: adjoint of obs_{k+1}
 #pragma unroll
-          for (int j = 0; j < MAXA; ++j) zb[j] = abar[j] * g[j];
+          for (int j = 0; j < NA; ++j) zb[j] = abar[j] * g[j];
         }
       }
+      pr.stamp(kRevAdj);
       layer1_finish<true, AF>(G, P, d1, a1p);
-      layer2_back<true, false, AF>(G, P, zb, nullptr, acc3);
+      pr.stamp(kRevL1);
+      layer2_back<true, false, AF, NA>(G, P, zb, nullptr, acc3);
+      pr.stamp(kRevL2);
       float dx[NS];
-      backprop<true, NS>(G, P, k > 0, part, G.X(k), a1p, dx);
+      backprop<true, NS, NA == 1>(G, P, k > 0, part, G.X(k), a1p, dx, pr);
       if (active && k > 0) {                          // + the policy's input gradient of step k
 #pragma unroll
         for (int f = 0; f < NS; ++f)
           if (f < obs_dim) lam[f] += dx[f];
       }
+      pr.stamp(kRevD1);
+      pr.step(false);
     }
     wg::wg_sync(G.g);                                 // step 0's dW1 product has read its observation planes
   }
@@ -715,18 +757,18 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
   const int lane = G.t & 31, w4 = G.t >> 5;
   if (alg != ALG_TRACE) {
     const NetL& U = (alg == ALG_PEV) ? V : P;
-    constexpr int stride = MAXA * 64 + MAXA;
+    constexpr int stride = NA * 64 + NA;
     float* rg = reinterpret_cast<float*>(G.P);                         // [4 warps][stride]: the planes are dead
 #pragma unroll
-    for (int a = 0; a < MAXA; ++a)
-      if (a < U.out) {
+    for (int a = 0; a < NA; ++a)
+      if (live<NA>(a, U)) {
         const int col = 8 * (lane >> 2) + 2 * G.c;
         rg[w4 * stride + a * 64 + col] = acc3.w[a][0];
         rg[w4 * stride + a * 64 + col + 1] = acc3.w[a][1];
         float sb = acc3.b[a];                                          // owners' rows; 0 elsewhere
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) sb += __shfl_xor_sync(0xffffffffu, sb, o);
-        if (lane == 0) rg[w4 * stride + MAXA * 64 + a] = sb;
+        if (lane == 0) rg[w4 * stride + NA * 64 + a] = sb;
       }
     wg::wg_sync(G.g);
     for (int i = G.t; i < U.out * 64; i += 128) {
@@ -734,8 +776,8 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
       part[U.g_w3 + i] = (rg[a * 64 + j] + rg[stride + a * 64 + j]) + (rg[2 * stride + a * 64 + j] + rg[3 * stride + a * 64 + j]);
     }
     if (G.t < U.out)
-      part[U.g_b3 + G.t] = (rg[MAXA * 64 + G.t] + rg[stride + MAXA * 64 + G.t]) +
-                           (rg[2 * stride + MAXA * 64 + G.t] + rg[3 * stride + MAXA * 64 + G.t]);
+      part[U.g_b3 + G.t] = (rg[NA * 64 + G.t] + rg[stride + NA * 64 + G.t]) +
+                           (rg[2 * stride + NA * 64 + G.t] + rg[3 * stride + NA * 64 + G.t]);
     wg::wg_sync(G.g);
   }
   {  // the three scalars of the sub-tile slot (fixed order over its 64 rows; only owner threads carry values)
@@ -749,6 +791,7 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
       part[nparam + G.t] = s;
     }
   }
+  pr.finish(alg, WGS);
 }
 
 }  // namespace gops
