@@ -5,16 +5,18 @@
 //   registers: thread t (warp w = t / 32, lane l) holds rows 16 w + l / 4 and 16 w + l / 4 + 8, columns 8 j + 2 (l % 4)
 //   + {0, 1} (wgmma.cuh).  Bias, activation, act', the split into bf16 planes, the output layer (summed over the four
 //   lanes of a quad by shuffles), delta2 = act'(pre2) * (W3^T zbar) and delta1 = (delta2 . W2) * act'(pre1) are all
-//   computed on that fragment; act'(layer 1) stays in registers from the recompute until delta1 is formed.
+//   computed on that fragment; act'(layer 1) stays in registers from the recompute until delta1 is formed.  The m64n64
+//   accumulator fragment is the register-A fragment of the next m64nNk16 product (k-step ks = registers 8 ks .. 8 ks + 7),
+//   so a forward-only layer 2 takes its three bf16 A planes straight from the layer-1 fragment, without shared memory.
 //   Lanes 4q and 4q + 1 of warp w own rows 16 w + q and 16 w + q + 8: they keep the sample's model state and adjoint for
 //   the whole horizon, run the dynamics / adjoint and write the observation row into the operand planes.  z, zbar and
 //   the input gradient move within the quad by shuffles.
 //
 //   The reductions over samples run on the tensor core as well (MN-major view of the same operand planes, K = 64):
-//   dW2 / db2 / dW1 / db1 (db against a column of ones).  Each fragment is added into the warpgroup's own FP32 global
-//   partial with red.global.add: every address of a partial has one writing thread, which adds in program order, so
-//   the gradient is bit-reproducible, and no load sits on the critical path.  dW3 / db3 are shuffle / register sums,
-//   written once at the end.
+//   dW2 / db2 / dW1 / db1 (db against a column of ones).  dW2 is added into the warpgroup's FP32 sum in shared memory
+//   (add.rn.ftz: the rounding of red.global.add.f32) and written to its global partial once, at the end; dW1, db2 and
+//   db1 are added into the partial with red.global.add.  Every address has one writing thread, which adds in program
+//   order, so the gradient is bit-reproducible.  dW3 / db3 are shuffle / register sums, written once at the end.
 //
 // Synchronisation: a warpgroup meets only itself (128-thread named barrier, fence.proxy.async before a wgmma reads
 // planes the threads just wrote).  FHADP has no CTA-wide barrier after the initial weight stage; INFADP swaps weight
@@ -26,9 +28,9 @@
 //   delta / input grad    delta . W    delta in TWO bf16 planes (2^-17 relative: the gradient bar is 2e-4), W in three
 //   weight gradients      delta^T . h  (delta_b0 + delta_b1) . (h_b0 + h_b1): four terms, FP32 accumulation
 //
-// Shared memory (~188 KB of 227 with three warpgroups): weights 31.5 KB (TMA-staged), ones 0.5 KB, and per warpgroup
-// H1 planes 24 KB, delta planes 16 KB (delta2, then delta1 in the same buffer), observation planes 2 x 6 KB (double
-// buffered by horizon step: the dW1 product of step k still reads step k's rows while step k - 1 writes its own).
+// Shared memory (~218 KB of 227 with three warpgroups): weights 31.5 KB (TMA-staged), ones 0.5 KB, and per warpgroup
+// H1 planes 24 KB, delta planes 16 KB (delta2, then delta1 in the same buffer), observation planes 6 KB (one buffer:
+// put_x meets the warpgroup before it overwrites rows the last wgmma may still read) and the FP32 sum of dW2 16 KB.
 #pragma once
 #include "models.cuh"
 #include "mlp_tc_full.cuh"
@@ -42,7 +44,8 @@ constexpr int GT = 64;                  // rows (= samples) per sub-tile = wgmma
 constexpr int NT2 = 128 * WGS;          // threads per CTA
 constexpr int HPL = tcf::HPLANE, XPL = tcf::XPLANE;
 constexpr int P_BYTES = 3 * HPL, Q_BYTES = 2 * HPL, XP_BYTES = 3 * XPL;
-constexpr int GROUP_BYTES = P_BYTES + Q_BYTES + 2 * XP_BYTES;
+constexpr int ACC_BYTES = 64 * 64 * 4;  // FP32 dW2 sum, in fragment order (acc_frag)
+constexpr int GROUP_BYTES = P_BYTES + Q_BYTES + XP_BYTES + ACC_BYTES;
 constexpr int HDR_BYTES = 256;
 
 __host__ __device__ inline size_t smem_bytes(int w_floats) {
@@ -62,19 +65,23 @@ __device__ __forceinline__ void split2(f32x2::u64 X, uint32_t& p0, uint32_t& p1)
 __device__ __forceinline__ void red_add(float* p, float v) {
   asm volatile("red.global.add.f32 [%0], %1;" ::"l"(p), "f"(v) : "memory");
 }
-__device__ __forceinline__ void red_add2(float* p, float v0, float v1) {   // 8-byte aligned pair
-  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(v0), "f"(v1) : "memory");
+// a + b rounded as red.global.add.f32 rounds: to nearest even, subnormal inputs and result flushed to signed zero
+__device__ __forceinline__ float add_ftz(float a, float b) {
+  float r;
+  asm("add.rn.ftz.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
 }
 
 // Per-thread view of its warpgroup's resources (kept small: everything else is an offset from P / Wsm).
 struct Grp {
-  unsigned char* P;                 // this warpgroup's planes: H1 (3) | delta (2) | observation (2 buffers of 3)
+  unsigned char* P;                 // this warpgroup's planes: H1 (3) | delta (2) | observation (3) | dW2 sum
   const float* Wsm;                 // staged weight blob of the network in use (NetL offsets); `ones` precedes it
   int g, t, c;                      // warpgroup, thread in the warpgroup, t % 4 (column pair of the fragment)
   int row;                          // owned row of the sub-tile (lanes 4q, 4q + 1 of a quad; see own)
   bool own;
   __device__ __forceinline__ unsigned char* Q() const { return P + P_BYTES; }
-  __device__ __forceinline__ unsigned char* X(int k) const { return P + P_BYTES + Q_BYTES + (k & 1) * XP_BYTES; }
+  __device__ __forceinline__ unsigned char* X() const { return P + P_BYTES + Q_BYTES; }
+  __device__ __forceinline__ float* acc() const { return reinterpret_cast<float*>(P + P_BYTES + Q_BYTES + XP_BYTES); }
   __device__ __forceinline__ const unsigned char* ones() const {
     return reinterpret_cast<const unsigned char*>(Wsm) - tcf::ONES_B;
   }
@@ -110,6 +117,26 @@ __device__ __forceinline__ void mma6(float* d, const tcf::Op& A, const tcf::Op& 
   for (int ks = 0; ks < KS; ++ks) wg::mma_bf16<N, 0, TB>(d, a0 + ks * ka, b1 + ks * kb, 1u);
 #pragma unroll
   for (int ks = 0; ks < KS; ++ks) wg::mma_bf16<N, 0, TB>(d, a0 + ks * ka, b0 + ks * kb, 1u);
+}
+// the same product with A from registers: a[p][4 ks .. 4 ks + 3] = plane p's words of k-step ks (wgmma.cuh), same six
+// terms in the same order as mma6; B K-major
+template <int KS>
+__device__ __forceinline__ void mma6_ra(float* d, const uint32_t (*a)[4 * KS], const tcf::Op& B) {
+  using namespace tcf;
+  const uint64_t b0 = dsc(B, 0), b1 = dsc(B, 1), b2 = dsc(B, 2);
+  const uint64_t kb = B.kadv >> 4;
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) wg::mma_bf16_n64_ra<0>(d, a[2] + 4 * ks, b0 + ks * kb, ks > 0 ? 1u : 0u);
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) wg::mma_bf16_n64_ra<0>(d, a[0] + 4 * ks, b2 + ks * kb, 1u);
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) wg::mma_bf16_n64_ra<0>(d, a[1] + 4 * ks, b1 + ks * kb, 1u);
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) wg::mma_bf16_n64_ra<0>(d, a[1] + 4 * ks, b0 + ks * kb, 1u);
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) wg::mma_bf16_n64_ra<0>(d, a[0] + 4 * ks, b1 + ks * kb, 1u);
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) wg::mma_bf16_n64_ra<0>(d, a[0] + 4 * ks, b0 + ks * kb, 1u);
 }
 // delta (2 planes, K-major A) x W (MN-major B): a1b0, a0b1, a0b0 -- small terms first.  The dropped terms (a1b1, a0b2)
 // are 2^-17 relative, the size of delta's own two-plane truncation.
@@ -156,35 +183,48 @@ __device__ __forceinline__ void frag_to_planes(unsigned char* buf, const Grp& G,
     if constexpr (NP == 3) *reinterpret_cast<uint32_t*>(buf + 2 * HPL + off) = w2;
   }
 }
-// a [64 output rows][N] weight-gradient fragment added into the FP32 partial (row stride ld, columns < ncols);
-// PAIRS: ld and dst even, so adjacent columns go as one 8-byte add
-template <int N, bool PAIRS>
+// a [64 output rows][N] weight-gradient fragment added into the FP32 partial (row stride ld, columns < ncols)
+template <int N>
 __device__ __forceinline__ void red_frag(float* __restrict__ dst, int ld, int ncols, const float* d, int t) {
 #pragma unroll
   for (int i = 0; i < N / 2; i += 2) {
     const int row = wg::frag_row(t, i), col = wg::frag_col(t, i);
-    if constexpr (PAIRS) {
-      red_add2(dst + row * ld + col, d[i], d[i + 1]);
-    } else {
-      if (col < ncols) red_add(dst + row * ld + col, d[i]);
-      if (col + 1 < ncols) red_add(dst + row * ld + col + 1, d[i + 1]);
-    }
+    if (col < ncols) red_add(dst + row * ld + col, d[i]);
+    if (col + 1 < ncols) red_add(dst + row * ld + col + 1, d[i + 1]);
   }
 }
-// column 0 of an m64n16 fragment (a product against the ones column) -> the bias gradient
-__device__ __forceinline__ void red_bias(float* __restrict__ dst, const float* d, const Grp& G) {
+// the m64n64 dW2 fragment added into this thread's own slots of the warpgroup's sum, kept in fragment order
+// ([16 register pairs][128 threads] of float2: a warp's lanes touch 256 contiguous bytes, no bank conflict)
+__device__ __forceinline__ void acc_frag(const Grp& G, const float* d) {
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) {
+    float2* s = reinterpret_cast<float2*>(G.acc()) + (i >> 1) * 128 + G.t;
+    float2 v = *s;
+    v.x = add_ftz(v.x, d[i]);
+    v.y = add_ftz(v.y, d[i + 1]);
+    *s = v;
+  }
+}
+// column 0 of an m64n16 fragment (a product against the ones column) -> the bias gradient.  (Summed in shared memory
+// like dW2, db2 / db1 made ptxas spill more in the fixed-chain kernel: 110 B / 84 B of spill stores instead of 60 B.)
+__device__ __forceinline__ void red_bias(const Grp& G, float* part, int off, const float* d) {
   if (G.c == 0) {
-    red_add(dst + wg::frag_row(G.t, 0), d[0]);
-    red_add(dst + wg::frag_row(G.t, 2), d[2]);
+    red_add(part + off + wg::frag_row(G.t, 0), d[0]);
+    red_add(part + off + wg::frag_row(G.t, 2), d[2]);
   }
 }
 
-// owner: this row's input (K1 = 16 values, zero padded) -> the three observation planes of buffer `x`.  nch = 1: the
-// inputs fit the first 8-feature chunk (idpendulum: 6 + time), the second chunk was zeroed once at kernel start.
+// owner: this row's input (K1 = 16 values, zero padded) -> the three observation planes.  nch = 1: the inputs fit the
+// first 8-feature chunk (idpendulum: 6 + time), the second chunk was zeroed once at kernel start.  Called by every
+// thread of the warpgroup: the planes have one buffer, and each warp waited on its own for the last wgmma that read
+// them (layer 1 of the forward step, dW1 of the reverse step), so the warpgroup meets before an owner overwrites its
+// row.
 template <int NS>
-__device__ __forceinline__ void put_x(const Grp& G, unsigned char* x, const NetL& L, const float* st, float vt) {
+__device__ __forceinline__ void put_x(const Grp& G, const NetL& L, const float* st, float vt) {
   using namespace tcf;
+  wg::wg_sync(G.g);
   if (!G.own) return;
+  unsigned char* x = G.X();
   float v[16];
 #pragma unroll
   for (int f = 0; f < 16; ++f) v[f] = (f < NS && f < L.obs) ? st[f < NS ? f : 0] : 0.f;
@@ -212,15 +252,15 @@ __device__ __forceinline__ void put_x(const Grp& G, unsigned char* x, const NetL
   if constexpr ((AF) >= 0) { M(AF); }       \
   else { GOPS_ACT_SWITCH(act, M) }
 
-// layer 1, issue: observation planes of buffer x . W1^T -> d (asynchronous; layer1_finish waits)
-__device__ __forceinline__ void layer1_issue(const Grp& G, const NetL& L, const unsigned char* x, float* d) {
+// layer 1, issue: observation planes . W1^T -> d (asynchronous; layer1_finish waits)
+__device__ __forceinline__ void layer1_issue(const Grp& G, const NetL& L, float* d) {
   using namespace tcf;
   publish(G);                                     // observation rows visible
   wg::fence();
-  mma6<64, 0, 1>(d, k_act(x, XPL), k_w(G.W1(L), W1PLANE));
+  mma6<64, 0, 1>(d, k_act(G.X(), XPL), k_w(G.W1(L), W1PLANE));
   wg::commit();
 }
-// layer 1, epilogue: + b1, activation -> H1 planes; FULL: act'(pre1) into a1p
+// layer 1, epilogue: + b1, activation -> d; FULL (a backward pass follows): act'(pre1) into a1p and d -> the H1 planes
 template <bool FULL, int AF>
 __device__ __forceinline__ void layer1_finish(const Grp& G, const NetL& L, float* d, float* a1p) {
   wg::wait<0>();
@@ -233,7 +273,7 @@ __device__ __forceinline__ void layer1_finish(const Grp& G, const NetL& L, float
   }
   GOPS_TC2_ACT_SWITCH(AF, L.hact, GOPS_TC2_A1)
 #undef GOPS_TC2_A1
-  frag_to_planes<3>(G.P, G, d);
+  if constexpr (FULL) frag_to_planes<3>(G.P, G, d);
 }
 
 // layer 2 product H1 . W2^T -> d (waited)
@@ -245,6 +285,20 @@ __device__ __forceinline__ void layer2_product(const Grp& G, const NetL& L, floa
   wg::commit();
   wg::wait<0>();
   wg::reg_fence<32>(d);
+}
+// the same product with A from registers: h = this thread's H1 fragment, split into three bf16 planes of A words
+__device__ __forceinline__ void layer2_product_ra(const Grp& G, const NetL& L, const float* h, float* d) {
+  using namespace tcf;
+  uint32_t a[3][16];
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) split3(h[i], h[i + 1], a[0][i >> 1], a[1][i >> 1], a[2][i >> 1]);
+  wg::fence();
+  mma6_ra<4>(d, a, k_w(G.W2(L), W2PLANE));
+  wg::commit();
+  wg::wait<0>();
+  wg::reg_fence<32>(d);
+#pragma unroll
+  for (int p = 0; p < 3; ++p) wg::reg_fence_u32<16>(a[p]);
 }
 // NA: the kernel's action count = length of the per-output arrays (z, zbar, S, Acc3).  Every net has at least one
 // output; with NA = 1 that is all of them (the host selects such a kernel only for nets with one output), so output a
@@ -288,11 +342,13 @@ __device__ __forceinline__ void output_layer(const Grp& G, const NetL& L, const 
   output_sum<NA>(G, L, S, z);
 }
 
-// layer 2 + output layer, forward only: the owner gets z[a] = b3[a] + W3[a] . act(H1 . W2^T + b2)
-template <int AF, int NA>
-__device__ __forceinline__ void layer2_out(const Grp& G, const NetL& L, float* z) {
+// layer 2 + output layer, forward only: the owner gets z[a] = b3[a] + W3[a] . act(H1 . W2^T + b2).  REGA: H1 from
+// this thread's fragment h (layer2_product_ra), else from the H1 planes
+template <int AF, int NA, bool REGA>
+__device__ __forceinline__ void layer2_out(const Grp& G, const NetL& L, const float* h, float* z) {
   float d[32];
-  layer2_product(G, L, d);
+  if constexpr (REGA) layer2_product_ra(G, L, h, d);
+  else layer2_product(G, L, d);
 #define GOPS_TC2_A2(A)                                \
   _Pragma("unroll") for (int i = 0; i < 32; i += 2)   \
       act_fwd_pair_t<A>(f32x2::add(f32x2::pk(d[i], d[i + 1]), f32x2::ld(G.b2(L) + wg::frag_col(G.t, i))), d[i], d[i + 1]);
@@ -386,14 +442,14 @@ __device__ __forceinline__ void layer2_back(const Grp& G, const NetL& L, const f
 }
 
 // delta2 planes -> delta1 = (delta2 . W2) * act'(pre1) (same planes, once the readers of delta2 retired) -> the owner's
-// input gradient dx (want_dx) and, WANT_DW, the weight gradients of both layers added into the partial `part`.
-// x: the observation planes of this step's layer 1.  pr: phase probe (tc2_probe.cuh), stamps the delta2 / dW2 part.
+// input gradient dx (want_dx) and, WANT_DW, the weight gradients of both layers: dW2 into the warpgroup's shared-memory
+// sum, the others added into the partial `part`.  pr: phase probe (tc2_probe.cuh), stamps the delta2 / dW2 part.
 // OVERLAP (WANT_DW): delta2 . W2 and the layer-2 weight gradients go out as two commit groups of one issue, and delta1
 // is formed while the second runs.  Its 40 accumulators are live across delta1, so only the NA = 1 kernels take it (with
 // MAXA outputs ptxas spills more).
 template <bool WANT_DW, int NS, bool OVERLAP>
 __device__ __forceinline__ void backprop(const Grp& G, const NetL& L, bool want_dx, float* __restrict__ part,
-                                         const unsigned char* x, const float* a1p, float* dx, Probe& pr) {
+                                         const float* a1p, float* dx, Probe& pr) {
   using namespace tcf;
   publish(G);                                     // delta2 planes visible
   // delta2 . W2 and the layer-2 weight gradients read only the delta2 and H1 planes
@@ -424,8 +480,8 @@ __device__ __forceinline__ void backprop(const Grp& G, const NetL& L, bool want_
     wg::wait<0>();
     wg::reg_fence<32>(w);
     wg::reg_fence<8>(wb);
-    red_frag<64, true>(part + L.g_w2, 64, 64, w, G.t);
-    red_bias(part + L.g_b2, wb, G);
+    acc_frag(G, w);
+    red_bias(G, part, L.g_b2, wb);
   }
   pr.stamp(kRevD2);
   wg::wg_sync(G.g);                               // every wgmma read of delta2 retired
@@ -439,7 +495,7 @@ __device__ __forceinline__ void backprop(const Grp& G, const NetL& L, bool want_
   }
   if constexpr (WANT_DW) {
     wg::fence();
-    mma_wgrad<16, 2>(w1, mn_act(G.Q(), HPL), mn_act(x, XPL));
+    mma_wgrad<16, 2>(w1, mn_act(G.Q(), HPL), mn_act(G.X(), XPL));
     mma_wgrad<16, 1>(wb1, mn_act(G.Q(), HPL), ones_op(G));
     wg::commit();
   }
@@ -447,8 +503,8 @@ __device__ __forceinline__ void backprop(const Grp& G, const NetL& L, bool want_
   if constexpr (WANT_DW) {
     wg::reg_fence<8>(w1);
     wg::reg_fence<8>(wb1);
-    red_frag<16, false>(part + L.g_w1, L.in, L.in, w1, G.t);
-    red_bias(part + L.g_b1, wb1, G);
+    red_frag<16>(part + L.g_w1, L.in, L.in, w1, G.t);
+    red_bias(G, part, L.g_b1, wb1);
   }
   if (want_dx) {
     wg::reg_fence<8>(d);
@@ -545,7 +601,8 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
   Probe pr;
   pr.init(G.t);
 
-  for (int i = G.t; i < 2 * XP_BYTES / 16; i += 128) reinterpret_cast<uint4*>(G.X(0))[i] = make_uint4(0u, 0u, 0u, 0u);
+  // the observation planes and the dW2 sum that follows them
+  for (int i = G.t; i < (XP_BYTES + ACC_BYTES) / 16; i += 128) reinterpret_cast<uint4*>(G.X())[i] = make_uint4(0u, 0u, 0u, 0u);
   stage(p.blob_pol, P.blob);      // (its leading CTA barrier also publishes the zeroed planes)
 
   const long long nsub = (B + GT - 1) / GT;
@@ -583,11 +640,11 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           }
         }
         float z[NA], d1[32];
-        put_x<NS>(G, G.X(k), P, st, (float)(k + 1));
-        layer1_issue(G, P, G.X(k), d1);
+        put_x<NS>(G, P, st, (float)(k + 1));
+        layer1_issue(G, P, d1);
         layer1_finish<false, AF>(G, P, d1, nullptr);
         pr.stamp(kFwdL1);
-        layer2_out<AF, NA>(G, P, z);
+        layer2_out<AF, NA, true>(G, P, d1, z);
         pr.stamp(kFwdL2);
         if (own) {
           float a[NA], g[NA], apol[NA];
@@ -633,14 +690,14 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
         float zv[NA], zb[NA], d1[32], a1p[32];
 #pragma unroll
         for (int j = 0; j < NA; ++j) zb[j] = zv[j] = 0.f;
-        put_x<NS>(G, G.X(0), V, st, 0.f);
-        layer1_issue(G, V, G.X(0), d1);
+        put_x<NS>(G, V, st, 0.f);
+        layer1_issue(G, V, d1);
         if (alg == ALG_PIM) {
           float dx[NS];
           zb[0] = term ? -gn * p.inv_B : 0.f;
           layer1_finish<true, AF>(G, V, d1, a1p);
           layer2_back<false, true, AF, NA>(G, V, zb, zv, acc3);
-          backprop<false, NS, NA == 1>(G, V, true, part, G.X(0), a1p, dx, pr);
+          backprop<false, NS, NA == 1>(G, V, true, part, a1p, dx, pr);
           if (term) {
 #pragma unroll
             for (int f = 0; f < NS; ++f)
@@ -648,7 +705,7 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           }
         } else {
           layer1_finish<false, AF>(G, V, d1, nullptr);
-          layer2_out<AF, NA>(G, V, zv);
+          layer2_out<AF, NA, true>(G, V, d1, zv);
         }
         if (term) vacc += gn * zv[0];
       }
@@ -665,10 +722,10 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
 #pragma unroll
         for (int j = 0; j < NA; ++j) zb[j] = zv[j] = 0.f;
         // the output adjoint needs v(o_0) first: forward to the output, then recompute layer 2 fused with the backward
-        put_x<NS>(G, G.X(0), V, o0, 0.f);
-        layer1_issue(G, V, G.X(0), d1);
+        put_x<NS>(G, V, o0, 0.f);
+        layer1_issue(G, V, d1);
         layer1_finish<true, AF>(G, V, d1, a1p);
-        layer2_out<AF, NA>(G, V, zv);
+        layer2_out<AF, NA, false>(G, V, d1, zv);        // from the H1 planes, which layer2_back reads again
         if (valid) {
           const float diff = zv[0] - vacc;
           loss_acc += diff * diff * p.inv_B;
@@ -676,7 +733,7 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           zb[0] = 2.f * diff * p.inv_B;
         }
         layer2_back<true, false, AF, NA>(G, V, zb, nullptr, acc3);
-        backprop<true, NS, NA == 1>(G, V, false, part, G.X(0), a1p, nullptr, pr);
+        backprop<true, NS, NA == 1>(G, V, false, part, a1p, nullptr, pr);
       }
       stage(p.blob_pol, P.blob);
       continue;
@@ -711,8 +768,8 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           if (j < pout) zt[j] = tape[(k * TCH + NS + 1 + j) * GT + G.row];
       }
       float d1[32], a1p[32];
-      put_x<NS>(G, G.X(k), P, st, (float)(k + 1));
-      layer1_issue(G, P, G.X(k), d1);                // recompute of step k's layer 1, overlapped with the adjoint
+      put_x<NS>(G, P, st, (float)(k + 1));
+      layer1_issue(G, P, d1);                        // recompute of step k's layer 1, overlapped with the adjoint
       pr.stamp(kRevL1);
       float zb[NA];
 #pragma unroll
@@ -740,7 +797,7 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
       layer2_back<true, false, AF, NA>(G, P, zb, nullptr, acc3);
       pr.stamp(kRevL2);
       float dx[NS];
-      backprop<true, NS, NA == 1>(G, P, k > 0, part, G.X(k), a1p, dx, pr);
+      backprop<true, NS, NA == 1>(G, P, k > 0, part, a1p, dx, pr);
       if (active && k > 0) {                          // + the policy's input gradient of step k
 #pragma unroll
         for (int f = 0; f < NS; ++f)
@@ -749,7 +806,6 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
       pr.stamp(kRevD1);
       pr.step(false);
     }
-    wg::wg_sync(G.g);                                 // step 0's dW1 product has read its observation planes
   }
 
   // ============================ per-warpgroup partials ============================
@@ -757,6 +813,11 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
   const int lane = G.t & 31, w4 = G.t >> 5;
   if (alg != ALG_TRACE) {
     const NetL& U = (alg == ALG_PEV) ? V : P;
+    // the dW2 sum: each thread its own fragment
+#pragma unroll
+    for (int i = 0; i < 32; i += 2)
+      *reinterpret_cast<float2*>(part + U.g_w2 + wg::frag_row(G.t, i) * 64 + wg::frag_col(G.t, i)) =
+          reinterpret_cast<const float2*>(G.acc())[(i >> 1) * 128 + G.t];
     constexpr int stride = NA * 64 + NA;
     float* rg = reinterpret_cast<float*>(G.P);                         // [4 warps][stride]: the planes are dead
 #pragma unroll

@@ -1,6 +1,6 @@
 // Hopper (sm_90a) warpgroup tensor-core primitives: shared-memory matrix descriptors, wgmma.mma_async issue for BF16
-// (m64nNk16, N = 16 / 32 / 64 / 128) and TF32 (m64n64k8) with FP32 register accumulators, the fence / commit / wait of
-// the async group, and the fp32 -> TF32 hi / lo split.
+// (m64nNk16, N = 16 / 32 / 64 / 128; for N = 64 also with A from registers) and TF32 (m64n64k8) with FP32 register
+// accumulators, the fence / commit / wait of the async group, and the fp32 -> TF32 hi / lo split.
 //
 // Operand layout used throughout: the no-swizzle canonical layout, core matrix = 8 rows x 16 bytes.
 //   plane[kc][r][16 B]   r = 0..R-1 rows, kc = 16-byte column chunk
@@ -76,6 +76,25 @@ __device__ __forceinline__ void mma_bf16_n128(float* d, uint64_t a, uint64_t b, 
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB)
       : "memory");
+}
+
+// D (+)= A . B^T, m64n64k16, A from registers: four b32 words of packed bf16 pairs per thread, in the accumulator
+// fragment's order (a[0] row r, columns 2c + {0, 1}; a[1] row r + 8; a[2], a[3] the same rows, columns 8 + 2c + {0, 1};
+// r = 16 w + l / 4, c = l % 4).  The words are read asynchronously: they must stay unmodified until the wait.
+template <int TB>
+__device__ __forceinline__ void mma_bf16_n64_ra(float* d, const uint32_t* a, uint64_t b, uint32_t acc) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc), "n"(TB)
+      : "memory");
+}
+// keeps register-A words live (and unmoved) until after the wait that retires the wgmma reading them
+template <int N>
+__device__ __forceinline__ void reg_fence_u32(uint32_t* a) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(a[i])::"memory");
 }
 
 __device__ __forceinline__ void mma_tf32_n64(float* d, uint64_t a, uint64_t b, uint32_t acc) {
