@@ -333,7 +333,8 @@ int launch_fused(gops_b200_plan* pl, KParams p, Route route, cudaStream_t st, fl
   const NetL& upd = (alg == ALG_PEV) ? p.val : p.pol;
   p.part_stride = round4(upd.nparam + 4);
   p.dw_floats = round4(upd.nacc);
-  p.tape_ch = model_ns(pl->desc.model) + 1 + p.pol.out;
+  // tape columns per step: state, done flag, then per policy output z (mma.sync) or the action a and d a / d z (wgmma)
+  p.tape_ch = model_ns(pl->desc.model) + 1 + (tc ? 2 : 1) * p.pol.out;
   size_t smem;
   if (tc) {
     S = tc2::GT; NT = tc2::NT2; tape_cols = tc2::WGS * tc2::GT; rows = tc2::WGS;

@@ -129,8 +129,9 @@ __device__ __forceinline__ void wrapped_step(const KParams& p, int obs_dim, floa
 // Adjoint of wrapped_step for an active sample: st = outer observation before the step, lam = adjoint of the outer
 // observation after it (in) / before it (out), rho = dL/d(raw reward), abar[j] += dL/d a[j].  Chain of the step:
 //   obs_k -(1/scale, -shift)-> inner_0 -[model step x reps, same action]-> inner_reps -(+shift, *scale)-> clip -> obs_k+1
-// NA: length of abar (the kernel's action count; M reads a[0, NA) and writes at most MAXA adjoints).
-template <class M, int NA = MAXA, class W = WrapRt>
+// NA: length of abar (the kernel's action count; M reads a[0, NA) and writes at most MAXA adjoints).  UNROLL: passed to
+// M::step_bwd.
+template <class M, int NA = MAXA, class W = WrapRt, bool UNROLL = false>
 __device__ __forceinline__ void wrapped_step_bwd(const KParams& p, int obs_dim, const float* st, const float* a,
                                                  float rho, float* lam, float* abar) {
   constexpr int NS = M::NS;
@@ -164,7 +165,7 @@ __device__ __forceinline__ void wrapped_step_bwd(const KParams& p, int obs_dim, 
     const float rho_j = (W::repeat_num(p) == 0 || p.sum_reward || j == reps - 1) ? rho : 0.f;
 #pragma unroll
     for (int q = 0; q < MAXA; ++q) aj[q] = 0.f;
-    M::step_bwd(p, cur, a, rho_j, lam, aj);
+    M::template step_bwd<UNROLL>(p, cur, a, rho_j, lam, aj);
 #pragma unroll
     for (int q = 0; q < NA; ++q) abar[q] += aj[q];
   }
@@ -204,48 +205,62 @@ struct IdpAux {
   float i00, i01, i02, i11, i12, i22;  // symmetric inverse mass matrix
   float x0, x1, x2;                    // accelerations
 };
+// what the adjoint keeps of a sub-step's idp_eval: the MUFU sines / cosines and the IEEE reciprocal of det M
+struct IdpKeep {
+  float s1, c1, s2, c2, s12, c12, r;
+};
 
-__device__ __forceinline__ void idp_eval(const float* s, float u, const IdpC& c, IdpAux& q) {
-  // pendulum angles stay within a few radians: the MUFU sine/cosine (abs. error ~5e-7 on [-pi, pi]) is inside
-  // the fp32 noise of the reference here; the parity tests (loss 1e-4, gradient 2e-4, exact termination step) gate it
-  __sincosf(s[1], &q.s1, &q.c1);
-  __sincosf(s[2], &q.s2, &q.c2);
-  __sincosf(s[1] - s[2], &q.s12, &q.c12);
+// q from the sines / cosines in k and the angular velocities v1, v2.  FWD: forms k.r = 1 / det M, else takes it from k
+// (the same value: the mass matrix depends on the cosines alone)
+template <bool FWD>
+__device__ __forceinline__ void idp_eval_k(float v1, float v2, float u, const IdpC& c, IdpKeep& k, IdpAux& q) {
+  q.s1 = k.s1; q.c1 = k.c1; q.s2 = k.s2; q.c2 = k.c2; q.s12 = k.s12; q.c12 = k.c12;
   const float a = c.A, b = c.Bc * q.c1, cc = c.Cc * q.c2, d = c.D, e = c.E * q.c12, f = c.F;
-  const float v1 = s[4], v2 = s[5];
   const float f0 = (c.Bc * (v1 * v1)) * q.s1 + (c.Cc * (v2 * v2)) * q.s2 + u;
   const float f1 = (-c.E * (v2 * v2)) * q.s12 + c.G1 * q.s1;
-  const float f2 = (c.E * (v1 * v1)) * q.s12 + c.G2 * q.s2;
+  // rounded as written (as the compiler contracted it before q was kept): its choice depends on the other uses of q
+  const float f2 = __fmaf_rn(c.G2, q.s2, __fmul_rn(c.E * (v1 * v1), q.s12));
   const float C00 = d * f - e * e, C01 = cc * e - b * f, C02 = b * e - cc * d;
   const float C11 = a * f - cc * cc, C12 = b * cc - a * e, C22 = a * d - b * b;
-  const float det = a * C00 + b * C01 + cc * C02;
-  const float r = 1.f / det;
+  if constexpr (FWD) {
+    const float det = a * C00 + b * C01 + cc * C02;
+    k.r = 1.f / det;
+  }
+  const float r = k.r;
   q.i00 = C00 * r; q.i01 = C01 * r; q.i02 = C02 * r; q.i11 = C11 * r; q.i12 = C12 * r; q.i22 = C22 * r;
   q.x0 = q.i00 * f0 + q.i01 * f1 + q.i02 * f2;
   q.x1 = q.i01 * f0 + q.i11 * f1 + q.i12 * f2;
   q.x2 = q.i02 * f0 + q.i12 * f1 + q.i22 * f2;
 }
 
-__device__ __forceinline__ void idp_substep(float* s, float u, const IdpC& c) {
+// one sub-step in place; k receives what the adjoint keeps of it (IdpKeep)
+__device__ __forceinline__ void idp_substep(float* s, float u, const IdpC& c, IdpKeep& k) {
+  // pendulum angles stay within a few radians: the MUFU sine/cosine (abs. error ~5e-7 on [-pi, pi]) is inside
+  // the fp32 noise of the reference here; the parity tests (loss 1e-4, gradient 2e-4, exact termination step) gate it
+  __sincosf(s[1], &k.s1, &k.c1);
+  __sincosf(s[2], &k.s2, &k.c2);
+  __sincosf(s[1] - s[2], &k.s12, &k.c12);
   IdpAux q;
-  idp_eval(s, u, c, q);
+  idp_eval_k<true>(s[4], s[5], u, c, k, q);
   const float t = c.tau;
   const float n0 = s[0] + t * s[3], n1 = s[1] + t * s[4], n2 = s[2] + t * s[5];
   s[3] += t * q.x0; s[4] += t * q.x1; s[5] += t * q.x2;
   s[0] = n0; s[1] = n1; s[2] = n2;
 }
 
-// adjoint of one sub-step: lam (adjoint of s_next) -> lam (adjoint of s); ubar += dL/du
-__device__ __forceinline__ void idp_substep_bwd(const float* s, float u, const IdpC& c, float* lam, float& ubar) {
-  IdpAux q;
-  idp_eval(s, u, c, q);
-  const float t = c.tau, v1 = s[4], v2 = s[5];
+// adjoint of one sub-step: lam (adjoint of s_next) -> lam (adjoint of s); ubar += dL/du.  v1, v2: s[4], s[5];
+// q: idp_eval of (s, u), the only other use of s
+__device__ __forceinline__ void idp_substep_bwd(float v1, float v2, const IdpAux& q, const IdpC& c, float* lam,
+                                                float& ubar) {
+  const float t = c.tau;
   const float xb0 = t * lam[3], xb1 = t * lam[4], xb2 = t * lam[5];
-  // w = M^-T xb (M symmetric) is the adjoint of f; the adjoint of M is -w x^T
+  // w = M^-T xb (M symmetric) is the adjoint of f; the adjoint of M is -w x^T.  w2 and m02 are rounded as written (as
+  // the compiler contracted them when q was formed in this function): its choice depends on where q comes from
   const float w0 = q.i00 * xb0 + q.i01 * xb1 + q.i02 * xb2;
   const float w1 = q.i01 * xb0 + q.i11 * xb1 + q.i12 * xb2;
-  const float w2 = q.i02 * xb0 + q.i12 * xb1 + q.i22 * xb2;
-  const float m01 = -(w0 * q.x1 + w1 * q.x0), m02 = -(w0 * q.x2 + w2 * q.x0), m12 = -(w1 * q.x2 + w2 * q.x1);
+  const float w2 = __fmaf_rn(q.i22, xb2, __fmaf_rn(q.i02, xb0, __fmul_rn(q.i12, xb1)));
+  const float m01 = -(w0 * q.x1 + w1 * q.x0), m02 = -__fmaf_rn(w0, q.x2, __fmul_rn(w2, q.x0));
+  const float m12 = -(w1 * q.x2 + w2 * q.x1);
   float th1b = m01 * (-c.Bc * q.s1) + m12 * (-c.E * q.s12);
   float th2b = m02 * (-c.Cc * q.s2) + m12 * (c.E * q.s12);
   // f0 = Bc v1^2 s1 + Cc v2^2 s2 + u
@@ -276,8 +291,9 @@ struct ModelIdp {
   __device__ static __forceinline__ void step(const KParams&, float* s, const float* a, float& rew, bool& done) {
     const IdpC c = idp_const();
     const float u = 500.f * a[0];
+    IdpKeep k;
 #pragma unroll 1
-    for (int j = 0; j < 5; ++j) idp_substep(s, u, c);
+    for (int j = 0; j < 5; ++j) idp_substep(s, u, c, k);
     const float dist = 0.f * (s[0] * s[0]) + 5.f * (s[1] * s[1]) + 10.f * (s[2] * s[2]);
     const float vel = 0.5f * (s[3] * s[3]) + 0.5f * (s[4] * s[4]) + 1.f * (s[5] * s[5]);
     rew = 10.f - dist - vel - a[0] * a[0];
@@ -285,19 +301,23 @@ struct ModelIdp {
     done = (tip_y <= 1.0f) || (fabsf(s[0]) >= 15.f);
   }
   // backward: s = state BEFORE the step, lam = adjoint of the next state (in) / of s (out),
-  // rho = dL/d(raw reward of this step).  abar[j] = dL/d a[j].
+  // rho = dL/d(raw reward of this step).  abar[j] = dL/d a[j].  UNROLL: the sub-step loops unrolled, so that what the
+  // adjoint keeps of each sub-step (45 floats in all) stays in registers; else they are rolled over thread-local arrays.
+  template <bool UNROLL = false>
   __device__ static __forceinline__ void step_bwd(const KParams&, const float* s, const float* a, float rho, float* lam,
                                                   float* abar) {
     const IdpC c = idp_const();
     const float u = 500.f * a[0];
-    float sj[5][6], s5[6];     // sub-step states: indexed in rolled loops (thread-local stack, L1 resident)
+    // what the adjoint of sub-step j needs of its state: the angular velocities and IdpKeep, formed once here
+    float vj[5][2], s5[6];
+    IdpKeep kj[5];
 #pragma unroll
     for (int f = 0; f < 6; ++f) s5[f] = s[f];
-#pragma unroll 1
+#pragma unroll (UNROLL ? 5 : 1)
     for (int j = 0; j < 5; ++j) {
-#pragma unroll
-      for (int f = 0; f < 6; ++f) sj[j][f] = s5[f];
-      idp_substep(s5, u, c);
+      vj[j][0] = s5[4];
+      vj[j][1] = s5[5];
+      idp_substep(s5, u, c, kj[j]);
     }
     // reward is evaluated on the post-step state
     lam[1] += rho * (-10.f * s5[1]);
@@ -306,8 +326,12 @@ struct ModelIdp {
     lam[4] += rho * (-s5[4]);
     lam[5] += rho * (-2.f * s5[5]);
     float ubar = 0.f;
-#pragma unroll 1
-    for (int j = 4; j >= 0; --j) idp_substep_bwd(sj[j], u, c, lam, ubar);
+#pragma unroll (UNROLL ? 5 : 1)
+    for (int j = 4; j >= 0; --j) {
+      IdpAux q;
+      idp_eval_k<false>(vj[j][0], vj[j][1], u, c, kj[j], q);
+      idp_substep_bwd(vj[j][0], vj[j][1], q, c, lam, ubar);
+    }
     abar[0] = rho * (-2.f * a[0]) + 500.f * ubar;
   }
 };
@@ -340,6 +364,7 @@ struct ModelLq {
     }
     done = false;
   }
+  template <bool = false>
   __device__ static __forceinline__ void step_bwd(const KParams& p, const float* s, const float* a, float rho,
                                                   float* lam, float* abar) {
     float tb[LQN];

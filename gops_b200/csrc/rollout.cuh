@@ -72,7 +72,8 @@ struct KParams {
   int ref_t, ref_len, veh_P;
   float veh_Pdt;           // fp32(pre_horizon * dt) as formed by the reference in python doubles
   // scratch
-  float* tape;             // [grid][H][tape_ch][NT]  (state, done flag, policy pre-activation z)
+  float* tape;             // [grid][H][tape_ch][NT]  (state, done flag, then per policy output: mma.sync the pre-activation
+                           // z; wgmma the action a and d a / d z)
   int tape_ch;
   float* ext_ref;          // veh3dofconti: [grid][P+1+H][4][NT] raw reference points (window slides by one per step)
   float* partial;          // [grid][part_stride]

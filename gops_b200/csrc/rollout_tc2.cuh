@@ -12,6 +12,9 @@
 //   the whole horizon, run the dynamics / adjoint and write the observation row into the operand planes.  z, zbar and
 //   the input gradient move within the quad by shuffles.
 //
+//   Tape (FHADP / PIM; the owner's row of its slot's columns): per step the state, the done flag, and per policy output
+//   the action a handed to the model and d a / d z, so that the reverse step neither re-reads z nor repeats the squash.
+//
 //   The reductions over samples run on the tensor core as well (MN-major view of the same operand planes, K = 64):
 //   dW2 / db2 / dW1 / db1 (db against a column of ones).  dW2 is added into the warpgroup's FP32 sum in shared memory
 //   (add.rn.ftz: the rounding of red.global.add.f32) and written to its global partial once, at the end; dW1, db2 and
@@ -648,12 +651,15 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
         pr.stamp(kFwdL2);
         if (own) {
           float a[NA], g[NA], apol[NA];
+          process_action<NA, W>(p, pout, z, a, g, apol);
           if (alg == ALG_FHADP || alg == ALG_PIM) {
 #pragma unroll
             for (int j = 0; j < NA; ++j)
-              if (j < pout) tape[(k * TCH + NS + 1 + j) * GT + G.row] = z[j];
+              if (j < pout) {
+                tape[(k * TCH + NS + 1 + j) * GT + G.row] = a[j];
+                tape[(k * TCH + NS + 1 + pout + j) * GT + G.row] = g[j];
+              }
           }
-          process_action<NA, W>(p, pout, z, a, g, apol);
           const bool active = valid && (p.mask_at_done ? !dn : true);
           float r = 0.f;
           if (valid) {
@@ -756,16 +762,19 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
     }
     for (int k = H - 1; k >= 0; --k) {
       pr.mark();
-      float zt[NA];
+      float a[NA], g[NA];                            // step k's action and d a / d z, from the forward sweep
       const bool dnk = ndn;
 #pragma unroll
       for (int f = 0; f < NS; ++f) st[f] = nst[f];
 #pragma unroll
-      for (int j = 0; j < NA; ++j) zt[j] = 0.f;
+      for (int j = 0; j < NA; ++j) a[j] = g[j] = 0.f;
       if (own) {
 #pragma unroll
         for (int j = 0; j < NA; ++j)
-          if (j < pout) zt[j] = tape[(k * TCH + NS + 1 + j) * GT + G.row];
+          if (j < pout) {
+            a[j] = tape[(k * TCH + NS + 1 + j) * GT + G.row];
+            g[j] = tape[(k * TCH + NS + 1 + pout + j) * GT + G.row];
+          }
       }
       float d1[32], a1p[32];
       put_x<NS>(G, P, st, (float)(k + 1));
@@ -782,11 +791,12 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           ndn = tape[((k - 1) * TCH + NS) * GT + G.row] != 0.f;
         }
         if (active) {
-          float a[NA], g[NA], abar[NA];
-          process_action<NA, W>(p, pout, zt, a, g, nullptr);
+          float abar[NA];
 #pragma unroll
           for (int j = 0; j < NA; ++j) abar[j] = 0.f;
-          wrapped_step_bwd<M, NA, W>(p, obs_dim, st, a, reward_adjoint(p, k), lam, abar);   // lam: adjoint of obs_{k+1}
+          // lam: adjoint of obs_{k+1}.  The NA = 1 kernel has the registers for an unrolled model adjoint; with MAXA
+          // outputs ptxas spills more
+          wrapped_step_bwd<M, NA, W, NA == 1>(p, obs_dim, st, a, reward_adjoint(p, k), lam, abar);
 #pragma unroll
           for (int j = 0; j < NA; ++j) zb[j] = abar[j] * g[j];
         }
