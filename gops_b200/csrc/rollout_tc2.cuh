@@ -10,7 +10,10 @@
 //   so a forward-only layer 2 takes its three bf16 A planes straight from the layer-1 fragment, without shared memory.
 //   Lanes 4q and 4q + 1 of warp w own rows 16 w + q and 16 w + q + 8: they keep the sample's model state and adjoint for
 //   the whole horizon, run the dynamics / adjoint and write the observation row into the operand planes.  z, zbar and
-//   the input gradient move within the quad by shuffles.
+//   the input gradient move within the quad by shuffles.  In the fixed-chain FHADP kernel (NA = 1) the forward sweep's
+//   layer 1 takes A from registers too (layer1_issue_ra): each lane of the quad gets the owners' inputs by shuffles
+//   and forms the bf16 words of its own feature pairs, so a forward step writes no observation planes and meets no
+//   barrier.  The reverse sweep still writes them: dW1 contracts over their MN-major view.
 //
 //   Tape (FHADP / PIM; the owner's row of its slot's columns): per step the state, the done flag, and per policy output
 //   the action a handed to the model and d a / d z, so that the reverse step neither re-reads z nor repeats the squash.
@@ -33,7 +36,8 @@
 //
 // Shared memory (~218 KB of 227 with three warpgroups): weights 31.5 KB (TMA-staged), ones 0.5 KB, and per warpgroup
 // H1 planes 24 KB, delta planes 16 KB (delta2, then delta1 in the same buffer), observation planes 6 KB (one buffer:
-// put_x meets the warpgroup before it overwrites rows the last wgmma may still read) and the FP32 sum of dW2 16 KB.
+// put_x meets the warpgroup before it overwrites rows the last wgmma may still read; the fixed-chain kernel's forward
+// sweep does not use them) and the FP32 sum of dW2 16 KB.
 #pragma once
 #include "models.cuh"
 #include "mlp_tc_full.cuh"
@@ -261,6 +265,42 @@ __device__ __forceinline__ void layer1_issue(const Grp& G, const NetL& L, float*
   publish(G);                                     // observation rows visible
   wg::fence();
   mma6<64, 0, 1>(d, k_act(G.X(), XPL), k_w(G.W1(L), W1PLANE));
+  wg::commit();
+}
+// the same product with A from registers (K = 16: one k-step), for a forward step that needs no observation planes.
+// Lane c of each quad takes the owners' inputs of both quad rows by shuffles and forms the split3 words of feature pairs
+// c and 4 + c (wgmma.cuh, mma_bf16_n64_ra) -- the words put_x stores for them -- then issues mma6's six terms in
+// mma6's order, so the result is bit-identical.  No shared memory, no barrier.  a: the A words, which the caller keeps
+// live (reg_fence_u32) until layer1_finish has waited.
+template <int NS>
+__device__ __forceinline__ void layer1_issue_ra(const Grp& G, const NetL& L, const float* st, float vt, float* d,
+                                                uint32_t (*a)[4]) {
+  using namespace tcf;
+  const int qb = (G.t & 31) & ~3;
+  float x[2][NS];                                 // the owners' state: row 16 w + q (lane 4q), row + 8 (lane 4q + 1)
+#pragma unroll
+  for (int r = 0; r < 2; ++r)
+#pragma unroll
+    for (int f = 0; f < NS; ++f) x[r][f] = __shfl_sync(0xffffffffu, st[f], qb + r);
+#pragma unroll
+  for (int r = 0; r < 2; ++r)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {                 // word 2 h + r: row r, features 8 h + 2 c + {0, 1}
+      float v[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int f = 8 * h + 2 * G.c + e;        // as put_x: the state (f < obs), the time input, else 0
+        float s = 0.f;
+#pragma unroll
+        for (int g = 0; g < NS; ++g)
+          if (g == f && g < L.obs) s = x[r][g];
+        if (L.time_input && f == L.in - 1) s = vt;
+        v[e] = s;
+      }
+      split3(v[0], v[1], a[0][2 * h + r], a[1][2 * h + r], a[2][2 * h + r]);
+    }
+  wg::fence();
+  mma6_ra<1>(d, a, k_w(G.W1(L), W1PLANE));
   wg::commit();
 }
 // layer 1, epilogue: + b1, activation -> d; FULL (a backward pass follows): act'(pre1) into a1p and d -> the H1 planes
@@ -544,6 +584,8 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
   static_assert(M::KIND == 0, "wgmma rollout kernel: state == obs models");
   static_assert(NA == 1 || NA == MAXA, "wgmma rollout kernel: NA is MAXA or 1");
   constexpr int NS = M::NS, alg = ALG;
+  // the fixed-chain FHADP kernel (NA = 1) feeds the forward sweep's layer 1 from registers (layer1_issue_ra)
+  constexpr bool kRegX1 = alg == ALG_FHADP && NA == 1;
   extern __shared__ __align__(16) float smem[];
   unsigned char* sm = reinterpret_cast<unsigned char*>(smem);
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm);           // [0] weights landed
@@ -643,9 +685,17 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           }
         }
         float z[NA], d1[32];
-        put_x<NS>(G, P, st, (float)(k + 1));
-        layer1_issue(G, P, d1);
-        layer1_finish<false, AF>(G, P, d1, nullptr);
+        if constexpr (kRegX1) {
+          uint32_t x1[3][4];
+          layer1_issue_ra<NS>(G, P, st, (float)(k + 1), d1, x1);
+          layer1_finish<false, AF>(G, P, d1, nullptr);
+#pragma unroll
+          for (int q = 0; q < 3; ++q) wg::reg_fence_u32<4>(x1[q]);
+        } else {
+          put_x<NS>(G, P, st, (float)(k + 1));
+          layer1_issue(G, P, d1);
+          layer1_finish<false, AF>(G, P, d1, nullptr);
+        }
         pr.stamp(kFwdL1);
         layer2_out<AF, NA, true>(G, P, d1, z);
         pr.stamp(kFwdL2);

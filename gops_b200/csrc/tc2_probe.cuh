@@ -16,7 +16,7 @@ namespace gops {
 namespace tc2 {
 
 enum Phase {
-  kFwdL1,    // forward step: observation planes, layer 1
+  kFwdL1,    // forward step: observation planes (fixed-chain kernel: A words in registers), layer 1
   kFwdL2,    // forward step: layer 2 + output layer
   kFwdDyn,   // forward step: action, wrapped model step, tape (owner lanes)
   kRevL1,    // reverse step: observation planes, layer 1 recompute (issue and epilogue)
