@@ -13,7 +13,9 @@
 //   the input gradient move within the quad by shuffles.  In the fixed-chain FHADP kernel (NA = 1) the forward sweep's
 //   layer 1 takes A from registers too (layer1_issue_ra): each lane of the quad gets the owners' inputs by shuffles
 //   and forms the bf16 words of its own feature pairs, so a forward step writes no observation planes and meets no
-//   barrier.  The reverse sweep still writes them: dW1 contracts over their MN-major view.
+//   barrier.  The reverse sweep still writes them: dW1 contracts over their MN-major view.  That kernel's reverse step
+//   feeds layer 2 from registers as well, and stores the same A words to the H1 planes for dW2 while the product runs,
+//   so no fence and barrier stand between the layer-1 epilogue and the layer-2 wgmma.
 //
 //   Tape (FHADP / PIM; the owner's row of its slot's columns): per step the state, the done flag, and per policy output
 //   the action a handed to the model and d a / d z, so that the reverse step neither re-reads z nor repeats the squash.
@@ -27,7 +29,12 @@
 // Synchronisation: a warpgroup meets only itself (128-thread named barrier, fence.proxy.async before a wgmma reads
 // planes the threads just wrote).  FHADP has no CTA-wide barrier after the initial weight stage; INFADP swaps weight
 // blobs (policy <-> v_target <-> v) through the one staging buffer, CTA-wide, so there all warpgroups of a CTA run the
-// same number of (possibly empty) sub-tile iterations.
+// same number of (possibly empty) sub-tile iterations.  Each warp waits only for its own share of a wgmma, so a plane
+// is rewritten only after a barrier that follows every warp's wait for the last product that read it.  The fixed-chain
+// kernel's reverse step meets five barriers, three of them after a proxy fence: put_x's, the layer-1 publish, the
+// delta2 publish, the barrier before delta1 is written and the delta1 publish.  Its H1 stores (during the layer-2
+// wgmma) follow the previous step's barrier before delta1, which follows that step's dW2 wait; the delta2 publish makes
+// them visible to this step's dW2.
 //
 // Arithmetic (bars: loss 1e-4, gradient 2e-4 against the CPU oracle):
 //   layer products        x . W^T      BF16x3 x BF16x3, six terms (FP32-accurate; the loss depends on these)
@@ -303,8 +310,9 @@ __device__ __forceinline__ void layer1_issue_ra(const Grp& G, const NetL& L, con
   mma6_ra<1>(d, a, k_w(G.W1(L), W1PLANE));
   wg::commit();
 }
-// layer 1, epilogue: + b1, activation -> d; FULL (a backward pass follows): act'(pre1) into a1p and d -> the H1 planes
-template <bool FULL, int AF>
+// layer 1, epilogue: + b1, activation -> d; FULL (a backward pass follows): act'(pre1) into a1p and, H1P, d -> the H1
+// planes
+template <bool FULL, int AF, bool H1P = FULL>
 __device__ __forceinline__ void layer1_finish(const Grp& G, const NetL& L, float* d, float* a1p) {
   wg::wait<0>();
   wg::reg_fence<32>(d);
@@ -316,7 +324,7 @@ __device__ __forceinline__ void layer1_finish(const Grp& G, const NetL& L, float
   }
   GOPS_TC2_ACT_SWITCH(AF, L.hact, GOPS_TC2_A1)
 #undef GOPS_TC2_A1
-  if constexpr (FULL) frag_to_planes<3>(G.P, G, d);
+  if constexpr (H1P) frag_to_planes<3>(G.P, G, d);
 }
 
 // layer 2 product H1 . W2^T -> d (waited)
@@ -329,7 +337,10 @@ __device__ __forceinline__ void layer2_product(const Grp& G, const NetL& L, floa
   wg::wait<0>();
   wg::reg_fence<32>(d);
 }
-// the same product with A from registers: h = this thread's H1 fragment, split into three bf16 planes of A words
+// the same product with A from registers: h = this thread's H1 fragment, split into three bf16 planes of A words.
+// H1P (a backward pass follows): the same words also go to the H1 planes for dW2, stored while the product runs (the
+// caller has met the warpgroup since the last wgmma that read them retired; the delta2 publish makes them visible)
+template <bool H1P = false>
 __device__ __forceinline__ void layer2_product_ra(const Grp& G, const NetL& L, const float* h, float* d) {
   using namespace tcf;
   uint32_t a[3][16];
@@ -338,6 +349,14 @@ __device__ __forceinline__ void layer2_product_ra(const Grp& G, const NetL& L, c
   wg::fence();
   mma6_ra<4>(d, a, k_w(G.W2(L), W2PLANE));
   wg::commit();
+  if constexpr (H1P) {
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {              // frag_to_planes<3>'s layout
+      const int off = (i >> 2) * (GT * 16) + wg::frag_row(G.t, i) * 16 + 4 * G.c;
+#pragma unroll
+      for (int p = 0; p < 3; ++p) *reinterpret_cast<uint32_t*>(G.P + p * HPL + off) = a[p][i >> 1];
+    }
+  }
   wg::wait<0>();
   wg::reg_fence<32>(d);
 #pragma unroll
@@ -458,11 +477,14 @@ __device__ __forceinline__ void delta2_epilogue(const Grp& G, const NetL& L, flo
 }
 
 // layer 2 recompute fused with the start of the backward pass: z for the owner (WANT_Z), dW3 / db3 sums, and
-// delta2 -> the two delta planes.  zbar: the owner's output adjoint of its row.
-template <bool WANT_DW, bool WANT_Z, int AF, int NA>
-__device__ __forceinline__ void layer2_back(const Grp& G, const NetL& L, const float* zbar, float* z, Acc3<NA>& acc3) {
+// delta2 -> the two delta planes.  zbar: the owner's output adjoint of its row.  REGA: H1 from this thread's fragment h
+// (layer2_product_ra, which also stores the H1 planes), else from the H1 planes
+template <bool WANT_DW, bool WANT_Z, int AF, int NA, bool REGA = false>
+__device__ __forceinline__ void layer2_back(const Grp& G, const NetL& L, const float* h, const float* zbar, float* z,
+                                            Acc3<NA>& acc3) {
   float d[32];
-  layer2_product(G, L, d);
+  if constexpr (REGA) layer2_product_ra<true>(G, L, h, d);
+  else layer2_product(G, L, d);
   const int qb = (G.t & 31) & ~3;
   float zr[2][NA];                                // zbar of the fragment's two rows
 #pragma unroll
@@ -584,8 +606,9 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
   static_assert(M::KIND == 0, "wgmma rollout kernel: state == obs models");
   static_assert(NA == 1 || NA == MAXA, "wgmma rollout kernel: NA is MAXA or 1");
   constexpr int NS = M::NS, alg = ALG;
-  // the fixed-chain FHADP kernel (NA = 1) feeds the forward sweep's layer 1 from registers (layer1_issue_ra)
-  constexpr bool kRegX1 = alg == ALG_FHADP && NA == 1;
+  // the fixed-chain FHADP kernel (NA = 1) feeds the forward sweep's layer 1 (layer1_issue_ra) and the reverse sweep's
+  // layer 2 (layer2_product_ra<true>) from registers
+  constexpr bool kRegA = alg == ALG_FHADP && NA == 1;
   extern __shared__ __align__(16) float smem[];
   unsigned char* sm = reinterpret_cast<unsigned char*>(smem);
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm);           // [0] weights landed
@@ -685,7 +708,7 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           }
         }
         float z[NA], d1[32];
-        if constexpr (kRegX1) {
+        if constexpr (kRegA) {
           uint32_t x1[3][4];
           layer1_issue_ra<NS>(G, P, st, (float)(k + 1), d1, x1);
           layer1_finish<false, AF>(G, P, d1, nullptr);
@@ -752,7 +775,7 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           float dx[NS];
           zb[0] = term ? -gn * p.inv_B : 0.f;
           layer1_finish<true, AF>(G, V, d1, a1p);
-          layer2_back<false, true, AF, NA>(G, V, zb, zv, acc3);
+          layer2_back<false, true, AF, NA>(G, V, nullptr, zb, zv, acc3);
           backprop<false, NS, NA == 1>(G, V, true, part, a1p, dx, pr);
           if (term) {
 #pragma unroll
@@ -788,7 +811,7 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
           vmean_acc += zv[0] * p.inv_B;
           zb[0] = 2.f * diff * p.inv_B;
         }
-        layer2_back<true, false, AF, NA>(G, V, zb, nullptr, acc3);
+        layer2_back<true, false, AF, NA>(G, V, nullptr, zb, nullptr, acc3);
         backprop<true, NS, NA == 1>(G, V, false, part, a1p, nullptr, pr);
       }
       stage(p.blob_pol, P.blob);
@@ -852,9 +875,10 @@ __global__ void __launch_bounds__(tc2::NT2, 1) rollout_tc2_kernel(const __grid_c
         }
       }
       pr.stamp(kRevAdj);
-      layer1_finish<true, AF>(G, P, d1, a1p);
+      // kRegA: layer 2 from this thread's layer-1 fragment, which goes to the H1 planes (for dW2) while it runs
+      layer1_finish<true, AF, !kRegA>(G, P, d1, a1p);
       pr.stamp(kRevL1);
-      layer2_back<true, false, AF, NA>(G, P, zb, nullptr, acc3);
+      layer2_back<true, false, AF, NA, kRegA>(G, P, d1, zb, nullptr, acc3);
       pr.stamp(kRevL2);
       float dx[NS];
       backprop<true, NS, NA == 1>(G, P, k > 0, part, a1p, dx, pr);

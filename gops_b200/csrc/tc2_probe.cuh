@@ -21,7 +21,8 @@ enum Phase {
   kFwdDyn,   // forward step: action, wrapped model step, tape (owner lanes)
   kRevL1,    // reverse step: observation planes, layer 1 recompute (issue and epilogue)
   kRevAdj,   // reverse step: wrapped model-step adjoint (owner lanes, overlapped with the layer-1 wgmma)
-  kRevL2,    // reverse step: layer 2 recompute + output, delta2 epilogue, dW3
+  kRevL2,    // reverse step: layer 2 recompute + output (fixed-chain kernel: A words in registers, stored to the H1
+             // planes after the issue), delta2 epilogue, dW3
   kRevD2,    // reverse step: delta2 . W2, dW2 / db2
   kRevD1,    // reverse step: delta1, input gradient, dW1 / db1
   kPhases
