@@ -74,6 +74,9 @@ PROTOTYPES = {
     "gops_b200_plan_set_path": (C.c_int, [C.c_void_p, C.c_int]),
     "gops_b200_plan_last_path": (C.c_int, [C.c_void_p]),
     "gops_b200_plan_set_constraint": (C.c_int, [C.c_void_p, C.c_int, C.c_float]),
+    "gops_b200_plan_set_spil_weights": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "gops_b200_spil_controller": (C.c_int, [C.c_void_p, C.c_int64, C.c_double, C.c_double, C.c_double, C.c_double,
+                                            C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gops_b200_plan_param_count": (C.c_int64, [C.c_void_p, C.c_int]),
     "gops_b200_rollout_grad": (C.c_int, [C.c_void_p, C.POINTER(Batch), C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -1,0 +1,201 @@
+"""Separated Proportional-Integral Lagrangian (SPIL), H100 edition.
+
+Same plugin surface as the reference (gops/algorithm/spil.py: ApproxContainer :32-70, SPIL :73-270): chance-constrained
+model-based RL on pyth_veh3dofconti_errcstr.  Every update runs both passes of the reference's `__compute_gradient`
+(:160-180), each as ONE fused CUDA kernel (csrc/kernel.cuh, constraint mode 4):
+
+  value pass   INFADP's PEV rollout (:182-212) without the (~d) mask on the terminal v_target, counting per constraint the
+               trajectories that stayed safe (constraint <= 0 on every step);
+  controller   `__spil_get_weight` (:257-270) as one device kernel in float64 that turns the batch's safe probability
+               into the weights [w_r, w_c0, w_c1] -- no host round trip;
+  policy pass  FHADP's differentiated rollout with the DetermPolicy (:214-255): -mean(w_r R + sum_i w_c,i prod_k Phi(c_k,i)),
+               the weights read from device memory;
+
+then both fused Adam steps and both Polyak averages (:146-158).  With several GPUs the value pass's safe counts are
+summed by the gradient exchange, so every rank runs the controller on the GLOBAL safe probability and the replicas keep
+identical multipliers (the reference's Ray replicas each run a controller of their own)."""
+__all__ = ["SPIL"]
+
+import time
+from copy import deepcopy
+from typing import Any, Tuple
+
+import numpy as np
+import torch
+
+from gops_b200 import _lib
+from gops_b200.algorithm.base import AlgorithmBase, ApprBase, FusedADPMixin
+from gops_b200.create_pkg.create_apprfunc import create_apprfunc
+from gops_b200.create_pkg.create_env_model import create_env_model
+from gops_b200.utils.common_utils import get_apprfunc_dict
+from gops_b200.utils.flat_params import GRAD_TAIL, FusedAdam, polyak_update
+from gops_b200.utils.tensorboard_setup import tb_tags
+
+MODE_SPIL = 4        # gops_b200_plan_set_constraint mode
+
+
+class ApproxContainer(ApprBase):
+    """v, policy and their Polyak targets + one fused Adam per trained network (spil.py:32-70)."""
+
+    def __init__(self, **kwargs):
+        super().__init__(**kwargs)
+        v_args = get_apprfunc_dict("value", **kwargs)
+        policy_args = get_apprfunc_dict("policy", **kwargs)
+        self.v = create_apprfunc(**v_args)
+        self.policy = create_apprfunc(**policy_args)
+        self.v_target = deepcopy(self.v)
+        self.policy_target = deepcopy(self.policy)
+        for p in self.v_target.parameters():
+            p.requires_grad = False
+        for p in self.policy_target.parameters():
+            p.requires_grad = False
+        self.policy_optimizer = FusedAdam(self.policy.flat_params, lr=kwargs["policy_learning_rate"])
+        self.v_optimizer = FusedAdam(self.v.flat_params, lr=kwargs["value_learning_rate"])
+        self.net_dict = {"v": self.v, "policy": self.policy}
+        self.target_net_dict = {"v": self.v_target, "policy": self.policy_target}
+        self.optimizer_dict = {"v": self.v_optimizer, "policy": self.policy_optimizer}
+        self.scheduler_dict = {}
+
+    def create_action_distributions(self, logits):
+        return self.policy.get_act_dist(logits)
+
+
+class SPIL(AlgorithmBase, FusedADPMixin):
+    """:param float gamma: discount factor.  :param float tau: Polyak coefficient of both targets.
+    :param int forward_step: model rollout length of both passes.  `pev_step` / `pim_step` are stored but unused, as in
+    the reference: both networks are updated on every iteration."""
+
+    def __init__(self, index: int = 0, gamma: float = 0.99, tau: float = 0.005, pev_step: int = 1, pim_step: int = 1,
+                 forward_step: int = 25, **kwargs: Any):
+        if kwargs.get("env_id") != "pyth_veh3dofconti_errcstr":
+            raise ValueError("SPIL is built for env_id='pyth_veh3dofconti_errcstr' (the fused kernel's constraint provider)")
+        if kwargs.get("constraint_dim") != 2:
+            raise ValueError("SPIL on pyth_veh3dofconti_errcstr needs constraint_dim=2 (|y_err| and |u_err| constraints)")
+        super().__init__(index, **kwargs)
+        self.networks = ApproxContainer(**kwargs)
+        self.envmodel = create_env_model(**kwargs)
+        self.gamma = gamma
+        self.tau = tau
+        self.pev_step = pev_step
+        self.pim_step = pim_step
+        self.forward_step = forward_step
+        self.reward_scale = 1.0        # hard-coded as in the reference; the reward_scale kwarg reaches ShapingReward only
+        self.n_constraint = kwargs["constraint_dim"]
+        self.Kp = 60
+        self.Ki = 0.02
+        self.Kd = 0
+        self.chance_thre = np.array([0.97] * self.n_constraint)
+        self.tb_info = dict()
+        self._init_fused()
+
+    @property
+    def adjustable_parameters(self):
+        return ("gamma", "tau", "pev_step", "pim_step", "forward_step", "reward_scale")
+
+    # ---- controller state (lives on the device) --------------------------------------------------------------------
+    def _ctl(self) -> Tuple[torch.Tensor, torch.Tensor]:
+        """float64 [delta_i(2), safe_prob_pre(2), lam(2)] and the policy pass's float32 weights [w_r, w_c0, w_c1]."""
+        if "_spil_state" not in self.__dict__:
+            dev = self._device()
+            self._spil_state = torch.zeros(6, dtype=torch.float64, device=dev)
+            self._spil_w = torch.zeros(3, dtype=torch.float32, device=dev)
+        return self._spil_state, self._spil_w
+
+    @property
+    def delta_i(self) -> np.ndarray:
+        return self._ctl()[0][0:2].cpu().numpy()
+
+    @delta_i.setter
+    def delta_i(self, value):
+        st = self._ctl()[0]
+        st[0:2] = torch.as_tensor(np.asarray(value, dtype=np.float64), device=st.device)
+
+    @property
+    def safe_prob(self) -> np.ndarray:
+        """safe probability of the most recent value pass (float32, as the reference's traj_issafe.mean(0))."""
+        return self._ctl()[0][2:4].cpu().numpy().astype(np.float32)
+
+    @property
+    def lam(self) -> np.ndarray:
+        return self._ctl()[0][4:6].cpu().numpy()
+
+    # ---- update ------------------------------------------------------------------------------------------------------
+    def local_update(self, data: dict, iteration: int) -> dict:
+        start_time = time.time()
+        nets = self.networks
+        tail_v = self._launch_and_step(lambda: self._value_pass(data), nets.v_optimizer)
+        self._controller(tail_v, data)
+        tail_p = self._launch_and_step(lambda: self._policy_pass(data), nets.policy_optimizer)
+        self._polyak()
+        self._publish(tail_v, tail_p, start_time)
+        return self.tb_info
+
+    def get_remote_update_info(self, data: dict, iteration: int) -> Tuple[dict, dict]:
+        start_time = time.time()
+        tail_v = self._value_pass(data)
+        self._controller(tail_v, data)
+        tail_p = self._policy_pass(data)
+        self._publish(tail_v, tail_p, start_time)
+        update_info = {name: [p.grad for p in self.networks.net_dict[name].parameters()] for name in ("v", "policy")}
+        return self.tb_info, update_info
+
+    def remote_update(self, update_info: dict):
+        for net_name, grads in update_info.items():
+            for p, grad in zip(self.networks.net_dict[net_name].parameters(), grads):
+                p.grad = grad
+        for net_name in update_info:
+            self.networks.optimizer_dict[net_name].step()
+        self._polyak(list(update_info))
+
+    def _polyak(self, names=("v", "policy")):
+        for name in names:
+            polyak_update(self.networks.target_net_dict[name].flat_params, self.networks.net_dict[name].flat_params,
+                          self.tau)
+
+    def _value_pass(self, data) -> torch.Tensor:
+        """loss_v and v's gradient; tail [loss_v | mean v | safe count 0 | safe count 1] (spil.py:182-212)."""
+        nets = self.networks
+        plan = self._plan(_lib.ALG_INFADP_VALUE, nets.policy, nets.v, self.forward_step, self.gamma)
+        _lib.check(_lib.lib().gops_b200_plan_set_constraint(plan.handle, MODE_SPIL, 1.0))
+        return self._rollout_grad(plan, data, nets.v.flat_params, nets.policy.flat_params, nets.v.flat_params,
+                                  nets.v_target.flat_params)
+
+    def _controller(self, tail_v: torch.Tensor, data):
+        """__spil_get_weight (spil.py:257-270) on the device; Kp / Ki / Kd / chance_thre are read on every call."""
+        thr = np.broadcast_to(np.asarray(self.chance_thre, dtype=np.float64), (2,))
+        batch = int(data["obs"].shape[0]) * self._world()[1]
+        state, weights = self._ctl()
+        with torch.cuda.device(state.device):
+            _lib.check(_lib.lib().gops_b200_spil_controller(
+                _lib.ptr(tail_v), batch, float(self.Kp), float(self.Ki), float(self.Kd), float(thr[0]), float(thr[1]),
+                _lib.ptr(state), _lib.ptr(weights), _lib.stream_ptr()))
+
+    def _policy_pass(self, data) -> torch.Tensor:
+        """loss_pi and the policy's gradient; tail [loss_pi | mean R | mean Phi product 0 | 1] (spil.py:214-255)."""
+        pol = self.networks.policy
+        plan = self._plan(_lib.ALG_FHADP, pol, None, self.forward_step, self.gamma)
+        _lib.check(_lib.lib().gops_b200_plan_set_constraint(plan.handle, MODE_SPIL, 1.0))
+        _lib.check(_lib.lib().gops_b200_plan_set_spil_weights(plan.handle, _lib.ptr(self._ctl()[1])))
+        return self._rollout_grad(plan, data, pol.flat_params, pol.flat_params, None, None)
+
+    def _publish(self, tail_v: torch.Tensor, tail_p: torch.Tensor, start_time: float):
+        """The update's one host read (honours loss_lag): both passes' tails in one pinned buffer."""
+        ring = self.__dict__.get("_spil_ring")
+        if ring is None:
+            ring = [(torch.zeros(2 * GRAD_TAIL, dtype=torch.float32).pin_memory(), torch.cuda.Event()) for _ in range(2)]
+            self.__dict__["_spil_ring"], self.__dict__["_spil_n"] = ring, 0
+        n = self.__dict__["_spil_n"]
+        buf, ev = ring[n % 2]
+        with torch.cuda.device(tail_v.device):
+            buf[:GRAD_TAIL].copy_(tail_v, non_blocking=True)
+            buf[GRAD_TAIL:].copy_(tail_p, non_blocking=True)
+            ev.record()
+        self.__dict__["_spil_n"] = n + 1
+        if self.loss_lag and n > 0:
+            buf, ev = ring[(n - 1) % 2]
+        ev.synchronize()
+        host = buf.tolist()
+        self.tb_info[tb_tags["loss_critic"]] = host[0]
+        self.tb_info[tb_tags["critic_avg_value"]] = host[1]
+        self.tb_info[tb_tags["loss_actor"]] = host[GRAD_TAIL]
+        self.tb_info[tb_tags["alg_time"]] = (time.time() - start_time) * 1000  # ms

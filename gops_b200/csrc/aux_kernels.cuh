@@ -78,6 +78,40 @@ __global__ void adam_kernel(float* __restrict__ p, const float* __restrict__ g, 
   v[i] = vi;
 }
 
+// SPIL's PI multiplier controller (spil.py:257-270), one thread per constraint, between the value and policy passes.
+// tail: the value pass's reduced scalars (slots 2 / 3 = safe trajectories of constraint 0 / 1, summed over ranks).
+// st: float64 [delta_i(2), safe_prob_pre(2), lam(2)], updated in place.  w: float32 [w_r, w_c0, w_c1] for the policy pass.
+// The float64 arithmetic is written with explicit _rn intrinsics (no FMA contraction) so that it equals the NumPy
+// expression bit for bit; safe_prob is a float32 mean and (safe_prob_pre - safe_prob) a float32 difference, as the
+// reference's float32 arrays make them, and Kd * delta_d is a float32 product (python scalar times a float32 array).
+__global__ void spil_controller_kernel(const float* __restrict__ tail, long long batch, double kp, double ki, float kd,
+                                       double thr0, double thr1, double* __restrict__ st, float* __restrict__ w) {
+  __shared__ double lam_s[2];
+  // np.clip: a NaN stays NaN
+  auto clip = [](double x, double hi) { return x < 0.0 ? 0.0 : (x > hi ? hi : x); };
+  const int i = threadIdx.x;
+  if (i < 2) {
+    const float sp = __fdiv_rn(tail[2 + i], (float)batch);
+    const double dp = __dadd_rn(i == 0 ? thr0 : thr1, -(double)sp);
+    const double adp = fabs(dp);
+    double sep = adp > 0.1 ? __dmul_rn(dp, 0.7) : dp;       // integral separation
+    if (adp > 0.2) sep = __dmul_rn(dp, 0.0);
+    const double di = clip(__dadd_rn(st[i], sep), 99999.0);
+    const float dd = (float)clip((double)__fsub_rn((float)st[2 + i], sp), 3333.0);
+    const double l = clip(__dadd_rn(__dadd_rn(__dmul_rn(ki, di), __dmul_rn(kp, dp)), (double)__fmul_rn(kd, dd)), 3333.0);
+    st[i] = di;
+    st[2 + i] = (double)sp;
+    st[4 + i] = l;
+    lam_s[i] = l;
+  }
+  __syncthreads();
+  if (i < 2) {
+    const double den = __dadd_rn(1.0, __dadd_rn(lam_s[0], lam_s[1]));
+    if (i == 0) w[0] = (float)__ddiv_rn(1.0, den);
+    w[1 + i] = (float)__ddiv_rn(lam_s[i], den);
+  }
+}
+
 __global__ void polyak_kernel(float* __restrict__ tgt, const float* __restrict__ src, float tau, long long n) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) tgt[i] = tgt[i] * (1.f - tau) + tau * src[i];

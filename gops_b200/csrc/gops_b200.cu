@@ -881,7 +881,19 @@ int gops_b200_plan_last_path(const gops_b200_plan* pl) { return pl ? pl->last_pa
 
 int gops_b200_plan_set_constraint(gops_b200_plan* pl, int mode, float coef) {
   if (!pl) return fail("null plan");
-  if (mode < 0 || mode > 3) return fail("unknown constraint mode");
+  if (mode < 0 || mode > 4) return fail("unknown constraint mode");
+  if (mode == 4) {
+    // SPIL runs on the mma.sync / FFMA rollout kernel only
+    if (!(pl->desc.model == GOPS_MODEL_VEH3DOFCONTI && pl->desc.veh_errcstr))
+      return fail("the SPIL constraint mode is built for pyth_veh3dofconti_errcstr only");
+    if (pl->desc.alg != GOPS_ALG_FHADP && pl->desc.alg != GOPS_ALG_INFADP_VALUE)
+      return fail("the SPIL constraint mode needs an FHADP (policy) or INFADP_VALUE (value) plan");
+    if (pl->desc.open_loop || pl->tc_ok || layerwise_built(pl))
+      return fail("the SPIL constraint mode is not built for the wgmma or layer-wise rollout paths");
+    pl->kp.cstr_mode = mode;
+    pl->kp.cstr_coef = 1.f;
+    return 0;
+  }
   const bool provider = (pl->desc.model == GOPS_MODEL_VEH3DOFCONTI && pl->desc.veh_errcstr) ||
                         (pl->desc.model == GOPS_MODEL_VEH3DOF_TRACKING && pl->desc.veh_detour);
   if (mode != 0 && !(provider && pl->desc.alg == GOPS_ALG_FHADP))
@@ -891,6 +903,26 @@ int gops_b200_plan_set_constraint(gops_b200_plan* pl, int mode, float coef) {
   pl->kp.cstr_mode = mode;
   pl->kp.cstr_coef = coef;
   return 0;
+}
+
+int gops_b200_plan_set_spil_weights(gops_b200_plan* pl, const float* weights) {
+  if (!pl) return fail("null plan");
+  pl->kp.spil_w = weights;
+  return 0;
+}
+
+int gops_b200_spil_controller(const float* tail, int64_t batch_global, double kp, double ki, double kd,
+                              double chance_thre0, double chance_thre1, double* state, float* weights, void* stream) {
+  ENTRY();
+  if (!tail || !state || !weights) return fail("null argument");
+  if (batch_global <= 0) return fail("empty batch");
+  const int dev = device_of(state);
+  if (dev < 0 || dev >= kMaxDevices) return fail("device index out of range");
+  DevGuard dg(dev);
+  spil_controller_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(tail, (long long)batch_global, kp, ki, (float)kd,
+                                                             chance_thre0, chance_thre1, state, weights);
+  ++g_launches;
+  return launched("launch#spil-controller");
 }
 
 int gops_b200_plan_launch_info(const gops_b200_plan* pl, int32_t* out4) {
@@ -932,6 +964,10 @@ int gops_b200_rollout_grad(gops_b200_plan* pl, const gops_b200_batch* b, const f
   cudaStream_t st = (cudaStream_t)stream;
   KParams p = bind_batch(pl, b, alg);
   p.inv_B = inv_batch_global;
+  if (p.cstr_mode == 4) {
+    if (route != Route::Mma) return fail("the SPIL constraint mode runs on the mma.sync rollout kernel only");
+    if (alg == GOPS_ALG_FHADP && !p.spil_w) return fail("SPIL policy pass: weights pointer not set (plan_set_spil_weights)");
+  }
   if (route == Route::Layerwise) return launch_layerwise(pl, p, policy_params, st, grad_out, scalars_out);
   if (launch_pack(pl, route, policy_params, false, pl->blob_pol.p, pl->blob_pol_tcf.p, st)) return 1;
   if (alg != GOPS_ALG_FHADP && launch_pack(pl, route, vtarget_params, true, pl->blob_vtg.p, pl->blob_vtg_tcf.p, st)) return 1;

@@ -5,6 +5,17 @@
 
 namespace gops {
 
+// SPIL's constraint-to-cost transform (spil.py:224-232): Phi(c) = (1 + tau m1) / (1 + m2 tau exp(clamp(c / tau, -10, 5)))
+// with m1 = 1, m2 = 0.45, tau = 0.07, constants formed in python doubles and applied to fp32 tensors.  dlog = d log Phi / dc
+// = -m2 e / (1 + m2 tau e) inside the clamp range, bounds included (torch's clamp passes the gradient there), else 0.
+__device__ __forceinline__ float spil_phi(float c, float& dlog) {
+  const float y = c / (float)0.07;
+  const float e = expf(fminf(fmaxf(y, -10.f), 5.f));
+  const float den = 1.f + (float)(0.45 * 0.07) * e;
+  dlog = (y >= -10.f && y <= 5.f) ? -0.45f * e / den : 0.f;
+  return (float)(1.0 + 0.07) / den;
+}
+
 // One CTA = NT threads = NT samples per chunk; MLP GEMMs run over SUB = NT/S sub-tiles of S samples that
 // reuse one set of activation tiles; the per-sample dynamics (forward and adjoint) run on every thread.
 // HD = 64: weights (TMA-staged), weight-gradient accumulators and X live in shared memory.
@@ -143,7 +154,9 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
     const long long gs = pos + col;
     bool dn = valid ? (p.done[gs] != 0.f) : true;
     float vacc = 0.f;
-    float cacc_a = 0.f, cacc_b = 0.f;            // constrained variants: discounted exterior|linear sum, interior (log) sum
+    // constrained variants: discounted exterior|linear sum, interior (log) sum; SPIL: per constraint the safe-so-far flag
+    // (value pass) or the running product of Phi (policy pass)
+    float cacc_a = p.cstr_mode == 4 ? 1.f : 0.f, cacc_b = cacc_a;
     bool infeasible = false;
     int path = 0, spd = 0;                       // vehicle models: reference path / speed profile ids
     RefWindow<M::KIND, NT> win;
@@ -207,10 +220,22 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
             bool inf;
 #pragma unroll
             for (int f = 0; f < 6; ++f) oc[f] = to_inner(p, f, t.X[f * XS + col]);
-            cstr_eval(oc, ce, cl, ci, inf);
-            cacc_a += (p.cstr_mode == 2 ? cl : ce) * p.gpow[k];
-            cacc_b += ci * p.gpow[k];
-            infeasible = infeasible || inf;
+            if (p.cstr_mode == 4) {
+              const float c0 = fabsf(oc[1]) - p.cstr_y_tol, c1 = fabsf(oc[3]) - p.cstr_u_tol;
+              if (alg == ALG_PEV) {          // traj_issafe *= constraint <= 0   (spil.py:200, 207)
+                cacc_a = c0 <= 0.f ? cacc_a : 0.f;
+                cacc_b = c1 <= 0.f ? cacc_b : 0.f;
+              } else {                       // c_mul = c_mul * Phi(constraint)  (spil.py:240-252)
+                float dl;
+                cacc_a *= spil_phi(c0, dl);
+                cacc_b *= spil_phi(c1, dl);
+              }
+            } else {
+              cstr_eval(oc, ce, cl, ci, inf);
+              cacc_a += (p.cstr_mode == 2 ? cl : ce) * p.gpow[k];
+              cacc_b += ci * p.gpow[k];
+              infeasible = infeasible || inf;
+            }
           }
         }
         if constexpr (M::KIND == 0) {
@@ -285,7 +310,8 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
     if (alg != ALG_FHADP) {
       stage(p.blob_vtg, V.blob);  // leading __syncthreads also publishes X = o_n
       const float gn = p.gpow[H];
-      const bool term = valid && !dn;
+      // SPIL's value target keeps gamma^n v_target(o_n) for done samples too (spil.py:209, no (~d) mask)
+      const bool term = valid && (!dn || (M::KIND == 1 && p.cstr_mode == 4));
       if (alg == ALG_PIM) {
         t.Z[col] = term ? -gn * p.inv_B : 0.f;     // row 0: d loss / d v_target(o_n); rows 1 (+5) receive v
         scope_sync();
@@ -317,6 +343,12 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
     }
 
     if (alg == ALG_PEV) {
+      if constexpr (M::KIND == 1) {
+        if (p.cstr_mode == 4 && valid) {     // SPIL: safe trajectories per constraint -> scalar tail slots 2 and 3
+          cint_acc += cacc_a;
+          feas_acc += cacc_b;
+        }
+      }
       // loss_v = mean((v(o_0) - backup)^2), gradient w.r.t. the value net only
       stage(p.blob_val, V.blob);
       load_obs_chunk(pos, nv, nsub * S);
@@ -342,10 +374,21 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
       continue;
     }
 
-    if (valid) loss_acc += -vacc * p.inv_B;
+    float ret = vacc;                    // the per-sample objective whose negated batch mean is the loss
+    if constexpr (M::KIND == 1) {
+      if (p.cstr_mode == 4 && valid) {
+        // SPIL: loss_pi = -mean(w_r R + sum_i w_c,i prod_k Phi(c_k,i))   (spil.py:253-255); tail [1] mean R,
+        // [2] / [3] mean Phi product of constraint 0 / 1
+        ret = p.spil_w[0] * vacc + (cacc_a * p.spil_w[1] + cacc_b * p.spil_w[2]);
+        vmean_acc += vacc * p.inv_B;
+        cint_acc += cacc_a * p.inv_B;
+        feas_acc += cacc_b * p.inv_B;
+      }
+    }
+    if (valid) loss_acc += -ret * p.inv_B;
     const bool feasible = !infeasible;
     if constexpr (M::KIND == 1) {
-      if (p.cstr_mode != 0 && valid) {
+      if (p.cstr_mode != 0 && p.cstr_mode != 4 && valid) {
         // exterior: penalty * mean(v_c); Lagrangian: multiplier * mean(v_c);
         // interior: mean(v_int * feasible) / penalty + penalty * mean(v_ext * ~feasible)   (fhadp_interior.py:78-84)
         float cl;
@@ -414,7 +457,10 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
 #pragma unroll
           for (int j = 0; j < MAXA; ++j) z[j] = j < P.out ? tape[(k * TCH + NS + 1 + j) * NT + tid] : 0.f;
           process_action(p, P.out, z, a, g, nullptr);
-          const float rho = reward_adjoint(p, k);
+          float rho = reward_adjoint(p, k);
+          if constexpr (M::KIND == 1) {
+            if (p.cstr_mode == 4) rho *= p.spil_w[0];     // SPIL: w_r weights the return
+          }
 #pragma unroll
           for (int j = 0; j < MAXA; ++j) abar[j] = 0.f;
           if constexpr (M::KIND == 0) {
@@ -453,7 +499,18 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
           const bool live = !(p.mask_at_done && dnk);
           float oc[6] = {0.f, live ? o6[1] : fz_y, 0.f, live ? o6[3] : fz_u, 0.f, 0.f};
           float gy, gu;
-          cstr_grad(oc, p.gpow[k] * p.inv_B, feasible, gy, gu);
+          if (p.cstr_mode == 4) {
+            // SPIL: d(-w_c,i / B prod_s Phi(c_s,i)) / dc_k,i = -w_c,i / B (prod_s Phi_s,i) dlog Phi(c_k,i); Phi >= 0.188, so
+            // the product over s != k is the total product over Phi_k
+            float d0, d1;
+            spil_phi(fabsf(oc[1]) - p.cstr_y_tol, d0);
+            spil_phi(fabsf(oc[3]) - p.cstr_u_tol, d1);
+            const float s0 = oc[1] > 0.f ? 1.f : (oc[1] < 0.f ? -1.f : 0.f), s1 = oc[3] > 0.f ? 1.f : (oc[3] < 0.f ? -1.f : 0.f);
+            gy = -p.spil_w[1] * p.inv_B * cacc_a * d0 * s0;
+            gu = -p.spil_w[2] * p.inv_B * cacc_b * d1 * s1;
+          } else {
+            cstr_grad(oc, p.gpow[k] * p.inv_B, feasible, gy, gu);
+          }
           gy += cbar_y; gu += cbar_u;
           if (made_here) {
             cbar_y = cbar_u = 0.f;
@@ -497,7 +554,8 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
   float* red = t.H1;  // free at this point, HID*(S+4) >= 3*NT floats
   red[tid] = loss_acc;
   red[NT + tid] = vmean_acc;
-  red[2 * NT + tid] = p.cstr_mode == 3 ? cint_acc : done_acc;     // interior point: the weighted log-barrier term
+  // interior point: the weighted log-barrier term; SPIL: safe count / mean Phi product of constraint 0
+  red[2 * NT + tid] = p.cstr_mode >= 3 ? cint_acc : done_acc;
   __syncthreads();
   if (tid < 3) {
     float s = 0.f;
@@ -505,7 +563,7 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
     part[nparam + tid] = s;
   }
   __syncthreads();
-  red[tid] = feas_acc;              // constrained variants: number of feasible samples (slot 3 of the scalar tail)
+  red[tid] = feas_acc;              // constrained variants: number of feasible samples (slot 3 of the scalar tail); SPIL: constraint 1
   __syncthreads();
   if (tid == 0) {
     float s = 0.f;

@@ -85,9 +85,11 @@ struct KParams {
   // trace outputs (alg == ALG_TRACE)
   float* tr_obs; float* tr_act; float* tr_rew; float* tr_done;
   // constrained FHADP variants (fhadp_exterior / fhadp_lagrangian / fhadp_interior.py): 0 none, 1 exterior penalty,
-  // 2 Lagrangian, 3 interior point; cstr_coef = penalty / multiplier; tolerances of the error-constraint vehicle model
+  // 2 Lagrangian, 3 interior point, 4 SPIL (spil.py: safe-trajectory counts on the value pass, the weighted
+  // Phi-product term on the policy pass); cstr_coef = penalty / multiplier; tolerances of the error-constraint model
   int cstr_mode;
   float cstr_coef, cstr_y_tol, cstr_u_tol;
+  const float* spil_w;     // cstr_mode 4, policy pass: device [w_r, w_c0, w_c1] written by the SPIL controller kernel
   // env_gen_ocp veh3dof_tracking_detour (lw_detour.cuh): surrounding-vehicle predictions [B][surr_len][1][5] (x, y, phi, u,
   // delta), circle offset d = (length - width) / 2 and 2 r = width of the bicircle collision model
   int veh_detour, surr_len;

@@ -30,7 +30,8 @@ class DeviceStateSampler:
         elif env_id == "pyth_lq":
             cfg = kwargs.get("lq_config", "s3a1")
             self._draw = lambda b: ds.sample_lq(b, cfg, self.device, gen=self.gen)
-        elif env_id == "pyth_veh3dofconti":
+        elif env_id in ("pyth_veh3dofconti", "pyth_veh3dofconti_errcstr"):
+            # the errcstr data env inherits pyth_veh3dofconti's reset law (pyth_veh3dofconti_errcstr.py:19)
             self._draw = lambda b: ds.sample_veh3dofconti(b, P, self.device, gen=self.gen)
         elif env_id == "veh3dof_tracking":
             self._draw = lambda b: ds.sample_veh3dof_tracking(b, P, self.device, gen=self.gen)

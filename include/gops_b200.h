@@ -174,8 +174,26 @@ int gops_b200_plan_last_path(const gops_b200_plan* plan);
  *   mode 3  interior point     loss = -mean(v_r) + mean(feasible * sum_k g^k sum_i log(-min(c_i,0) + 1e-8)) / coef
  *                                     + coef * mean(~feasible * sum_k g^k sum_i max(c_i,0)^2)     fhadp_interior.py:55-84
  * coef = penalty / multiplier of the CURRENT update (the algorithms anneal it on the host).  scalars_out of
- * rollout_grad then carries [0] total loss, [1] the exterior / linear constraint term (mean), [2] #done, [3] #feasible. */
+ * rollout_grad then carries [0] total loss, [1] the exterior / linear constraint term (mean), [2] #done, [3] #feasible.
+ *   mode 4  SPIL (gops/algorithm/spil.py), pyth_veh3dofconti_errcstr on the mma.sync kernel only (coef unused):
+ *     INFADP_VALUE plan  spil.py:182-212: loss_v = mean((v(o) - R)^2), R = sum_k g^k r_k + g^n v_target(o_n) WITHOUT the
+ *                        (~d) mask; scalars_out = [0] loss_v, [1] mean v(o), [2] / [3] number of trajectories whose
+ *                        constraint 0 / 1 stayed <= 0 on every step (the safe counts the controller turns into safe_prob).
+ *     FHADP plan         spil.py:214-255 (DetermPolicy, no terminal value): loss = -mean(w_r R + sum_i w_c,i prod_k
+ *                        Phi(c_k,i)), Phi(y) = 1.07 / (1 + 0.0315 exp(clamp(y / 0.07, -10, 5))); [w_r, w_c0, w_c1] are
+ *                        read from the device pointer of plan_set_spil_weights; scalars_out = [0] loss, [1] mean R,
+ *                        [2] / [3] mean Phi product of constraint 0 / 1.
+ * The wgmma and layer-wise rollout paths do not have mode 4: it is refused on plans that can take them. */
 int gops_b200_plan_set_constraint(gops_b200_plan* plan, int mode, float coef);
+/* SPIL policy pass: DEVICE pointer to float[3] = [w_r, w_c0, w_c1] (written by gops_b200_spil_controller), read by every
+ * later rollout_grad of this plan.  The pointer must stay valid while the plan uses it. */
+int gops_b200_plan_set_spil_weights(gops_b200_plan* plan, const float* weights);
+/* SPIL's PI multiplier controller (spil.py:257-270), one launch on `stream`, no host sync.  tail: DEVICE float[4] scalars of
+ * the value pass (after the gradient exchange, so slots 2 / 3 hold the global safe counts); batch_global: the global batch
+ * size.  safe_prob = float32(count) / float32(batch); state: DEVICE double[6] = [delta_i(2), safe_prob_pre(2), lam(2)],
+ * updated in place; weights: DEVICE float[3] = [w_r, w_c0, w_c1] = float32 of 1 / (1 + sum lam), lam / (1 + sum lam). */
+int gops_b200_spil_controller(const float* tail, int64_t batch_global, double kp, double ki, double kd,
+                              double chance_thre0, double chance_thre1, double* state, float* weights, void* stream);
 /* number of float32 parameters of the policy (which=0) / value (which=1) network */
 int64_t gops_b200_plan_param_count(const gops_b200_plan* plan, int which);
 
