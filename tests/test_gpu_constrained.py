@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 import torch
 
-from golden_util import inputs_from, load, rel_l2
+from golden_util import inputs_from, load, oracle_chunked, rel_l2
 from oracle import gops_oracle as orc
 
 pytestmark = pytest.mark.gpu
@@ -69,10 +69,15 @@ def test_two_updates_follow_the_reference(algname):
 @pytest.mark.parametrize("algname,mode", [("FHADPExterior", "exterior"), ("FHADPLagrangian", "lagrangian"),
                                           ("FHADPInterior", "interior")])
 def test_against_fp64_oracle_with_done_samples(algname, mode):
-    B = 777
+    check_against_fp64_oracle(algname, mode, 777)
+
+
+def check_against_fp64_oracle(algname, mode, B, seed=None):
+    """test_against_fp64_oracle_with_done_samples at any batch size (the oracle runs in chunks of 32768 samples); the
+    inputs are drawn with `seed` (default: B)."""
     torch.manual_seed(B)
     alg = _alg(algname, reward_scale=0.5)
-    data = orc.sample_inputs("pyth_veh3dofconti", B, seed=B, pre_horizon=10)
+    data = orc.sample_inputs("pyth_veh3dofconti", B, seed=B if seed is None else seed, pre_horizon=10)
     data["done"][::5] = 1.0
     env = orc.create_env_model("pyth_veh3dofconti_errcstr", dtype=torch.float64, pre_horizon=10, y_error_tol=1.2,
                                u_error_tol=2.2, reward_scale=0.5)
@@ -83,12 +88,24 @@ def test_against_fp64_oracle_with_done_samples(algname, mode):
                       time_input=True)
     coef = 2.0 if mode != "lagrangian" else 1.5
     d64 = {k: (v.double() if v.is_floating_point() else v) for k, v in data.items()}
-    loss, l_r, l_c, feas = orc.fhadp_constrained_loss(mode, pol, env, d64, 10, 0.97, coef)
-    loss.backward()
+    loss, ref_g, (l_r, l_c, feas) = oracle_chunked(
+        lambda d: orc.fhadp_constrained_loss(mode, pol, env, d, 10, 0.97, coef), d64, pol.params())
     tb = alg.get_remote_update_info(data, 0)[0]
-    assert abs(tb["Loss/Actor loss-RL iter"] - loss.item()) <= 1e-4 * max(1.0, abs(loss.item()))
-    assert abs(tb["Loss/Actor constraint loss-RL iter"] - l_c.item()) <= 1e-4 * max(1.0, abs(l_c.item()))
+    assert abs(tb["Loss/Actor loss-RL iter"] - loss) <= 1e-4 * max(1.0, abs(loss))
+    assert abs(tb["Loss/Actor constraint loss-RL iter"] - l_c) <= 1e-4 * max(1.0, abs(l_c))
+    bar = GRAD_RTOL
     if mode == "interior":
-        assert abs(tb["Loss/Feasible ratio-RL iter"] - float(feas)) < 1e-6
+        assert abs(tb["Loss/Feasible ratio-RL iter"] - feas) < 1e-6
+        # the log barrier amplifies the round-off of samples near the boundary (see above): noise floor = distance
+        # between the fp32 and the fp64 evaluation of the same oracle on this batch; the bar is three times that
+        env32 = orc.create_env_model("pyth_veh3dofconti_errcstr", dtype=torch.float32, pre_horizon=10, y_error_tol=1.2,
+                                     u_error_tol=2.2, reward_scale=0.5)
+        pol32 = orc.NetSpec([(w.detach().float().requires_grad_(True), b.detach().float().requires_grad_(True))
+                             for w, b in layers], "elu", "linear", torch.ones(2), -torch.ones(2), time_input=True)
+        _, g32, _ = oracle_chunked(lambda d: orc.fhadp_constrained_loss(mode, pol32, env32, d, 10, 0.97, coef), data,
+                                   pol32.params())
+        bar = max(GRAD_RTOL, 3.0 * rel_l2([g.numpy() for g in g32], [g.numpy() for g in ref_g]))
     got = [p.grad.detach().cpu().numpy() for p in alg.networks.policy.parameters()]
-    assert rel_l2(got, [t.grad.numpy() for pair in layers for t in pair]) < GRAD_RTOL
+    err = rel_l2(got, [g.numpy() for g in ref_g])
+    print(f"{algname} B={B}: gradient rel. L2 {err:.2e} (bar {bar:.2e})")
+    assert err < bar, (err, bar)

@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 import torch
 
-from golden_util import CASES, DEFAULT_LR, inputs_from, load, oracle_eval, rel_l2
+from golden_util import CASES, DEFAULT_LR, inputs_from, load, oracle_chunked, oracle_eval, rel_l2
 from oracle import gops_oracle as orc
 
 pytestmark = pytest.mark.gpu
@@ -214,6 +214,13 @@ def oracle_cases(cases):
 ]))
 def test_against_oracle_fp64(env_id, algname, act, B, H, wk):
     """Fresh seeded inputs, ragged batch sizes (not multiples of the tile), fp64 oracle as truth."""
+    check_against_oracle_fp64(env_id, algname, act, B, H, wk)
+
+
+def check_against_oracle_fp64(env_id, algname, act, B, H, wk):
+    """test_against_oracle_fp64 at any batch size: the oracle runs in chunks of 32768 samples, so that batches that
+    fill several chunks per CTA fit in host memory.  Returns the algorithm and, for FHADP, the oracle's number of samples
+    done at the end of the rollout."""
     from gops_b200.create_pkg.create_alg import create_alg
     hid = 256 if act.endswith("256") else 64
     act = act.replace("256", "")
@@ -260,32 +267,36 @@ def test_against_oracle_fp64(env_id, algname, act, B, H, wk):
         data["state"] = State(robot_state=robot, context_state=ContextState(reference=reference, t=t0))
     mk = _oracle_nets(alg, act, dt)
     pol = mk(alg.networks.policy, "pi", True)
+    n_done = None
     for it in ([0] if algname == "FHADP" else [0, 1]):
         if algname == "FHADP":
-            loss = orc.fhadp_loss(pol, env, d64, H, 0.98)
+            def chunk_loss(d):
+                trace = []
+                loss = orc.fhadp_loss(pol, env, d, H, 0.98, trace=trace)
+                return loss, trace[-1][3].double().mean()       # fraction done at the end of the rollout
             net, spec = "policy", pol
         elif it == 0:
             v, vt = mk(alg.networks.v, "v", False), mk(alg.networks.v_target, "v", False)
-            loss, _ = orc.infadp_loss_value(v, pol, vt, env, d64, H, 0.95)
+            chunk_loss = lambda d: orc.infadp_loss_value(v, pol, vt, env, d, H, 0.95)    # noqa: E731
             net, spec = "v", v
         else:
             vt = mk(alg.networks.v_target, "v", False)
-            loss = orc.infadp_loss_policy(pol, vt, env, d64, H, 0.95)
+            chunk_loss = lambda d: orc.infadp_loss_policy(pol, vt, env, d, H, 0.95)      # noqa: E731
             net, spec = "policy", pol
-        for p in spec.params():
-            p.grad = None
-        loss.backward()
+        ref_loss, ref_g, extras = oracle_chunked(chunk_loss, d64, spec.params())
         if algname == "FHADP":
+            n_done = round(extras[0] * B)
             alg._compute_gradient(data)
             got = alg.tb_info["Loss/Actor loss-RL iter"]
         else:
             alg.get_remote_update_info(data, it)
             got = alg.tb_info["Loss/Critic loss-RL iter" if it == 0 else "Loss/Actor loss-RL iter"]
         torch.cuda.synchronize()
-        assert abs(got - loss.item()) <= LOSS_RTOL * max(1.0, abs(loss.item())), (it, got, loss.item())
+        assert abs(got - ref_loss) <= LOSS_RTOL * max(1.0, abs(ref_loss)), (it, got, ref_loss)
         got_g = [p.grad.detach().cpu().numpy() for p in getattr(alg.networks, net).parameters()]
-        assert rel_l2(got_g, [p.grad.numpy() for p in spec.params()]) < GRAD_RTOL_BY_ENV.get(env_id, GRAD_RTOL), \
+        assert rel_l2(got_g, [g.numpy() for g in ref_g]) < GRAD_RTOL_BY_ENV.get(env_id, GRAD_RTOL), \
             (env_id, algname, it)
+    return alg, n_done
 
 
 def test_large_batch_properties():

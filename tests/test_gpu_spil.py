@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 import torch
 
-from golden_util import inputs_from, load, net_from, rel_l2
+from golden_util import inputs_from, load, net_from, oracle_chunked, rel_l2
 from oracle import gops_oracle as orc
 from oracle import spil_oracle as so
 
@@ -89,7 +89,12 @@ def test_four_updates_follow_the_reference(name):
 
 
 def test_against_fp64_oracle_with_done_samples():
-    B, y_tol, u_tol = 777, 2.0, 2.0
+    check_against_fp64_oracle(777)
+
+
+def check_against_fp64_oracle(B, y_tol=2.0, u_tol=2.0):
+    """test_against_fp64_oracle_with_done_samples at any batch size (the oracle runs in chunks of 32768 samples).
+    Returns the algorithm."""
     torch.manual_seed(B)
     alg = _alg(y_tol, u_tol, reward_scale=0.5)
     data = orc.sample_inputs("pyth_veh3dofconti", B, seed=B, pre_horizon=10)
@@ -105,30 +110,33 @@ def test_against_fp64_oracle_with_done_samples():
     tb, _ = alg.get_remote_update_info(_with_replay_keys(data), 0)
     torch.cuda.synchronize()
     # value pass
-    loss_v, vmean, issafe = so.spil_loss_value(v, pol, vt, env, d64, 10, 0.99)
-    loss_v.backward()
-    assert abs(tb[TB["loss_critic"]] - loss_v.item()) <= 1e-4 * max(1.0, abs(loss_v.item()))
-    assert abs(tb[TB["critic_avg_value"]] - vmean.item()) <= 1e-4 * max(1.0, abs(vmean.item()))
+    def value_chunk(d):
+        loss_v, vmean, issafe = so.spil_loss_value(v, pol, vt, env, d, 10, 0.99)
+        return (loss_v, vmean, *issafe.mean(0))
+    loss_v, g_v, (vmean, *safe) = oracle_chunked(value_chunk, d64, v.params())
+    assert abs(tb[TB["loss_critic"]] - loss_v) <= 1e-4 * max(1.0, abs(loss_v))
+    assert abs(tb[TB["critic_avg_value"]] - vmean) <= 1e-4 * max(1.0, abs(vmean))
     got = _grads(alg, "v")
     assert rel_l2([got[f"v.{2 * j}.{w}"] for j in range(3) for w in ("weight", "bias")],
-                  [t.grad.numpy() for pair in v.layers for t in pair]) < GRAD_RTOL
+                  [g.numpy() for g in g_v]) < GRAD_RTOL
     # safe counts: exact unless a constraint value lies within fp32 round-off of 0
     o, dn, info, near = d64["obs"], d64["done"], d64, torch.zeros(B, 2, dtype=torch.bool)
     with torch.no_grad():
         for _ in range(10):
             o, _, dn, info = env.forward(o, pol.act(o), dn, info)
             near |= info["constraint"].abs() < 1e-4
-    counts = issafe.sum(0).numpy()
-    got_counts = alg.safe_prob.astype(np.float64) * B
+    counts = np.array(safe) * B
+    got_counts = np.rint(alg.safe_prob.astype(np.float64) * B)      # safe_prob is a float32 ratio of counts
     assert np.all(np.abs(got_counts - counts) <= near.sum(0).numpy() + 1e-3), (got_counts, counts)
     # policy pass with the weights the controller left on the device
     w = alg._ctl()[1].cpu().numpy().astype(np.float64)
-    loss_pi = so.spil_loss_policy(pol, env, d64, 10, 0.99, w[0], w[1:])
-    loss_pi.backward()
-    assert abs(tb[TB["loss_actor"]] - loss_pi.item()) <= 1e-4 * max(1.0, abs(loss_pi.item()))
+    loss_pi, g_pi, _ = oracle_chunked(lambda d: so.spil_loss_policy(pol, env, d, 10, 0.99, w[0], w[1:]), d64,
+                                      pol.params())
+    assert abs(tb[TB["loss_actor"]] - loss_pi) <= 1e-4 * max(1.0, abs(loss_pi))
     got = _grads(alg, "policy")
     assert rel_l2([got[f"pi.{2 * j}.{w}"] for j in range(3) for w in ("weight", "bias")],
-                  [t.grad.numpy() for pair in pol.layers for t in pair]) < GRAD_RTOL
+                  [g.numpy() for g in g_pi]) < GRAD_RTOL
+    return alg
 
 
 @pytest.mark.parametrize("Kp,Ki,Kd", [(60, 0.02, 0), (60, 0.02, 0.5), (6000, 0.3, 1e4)])
