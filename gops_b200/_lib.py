@@ -128,6 +128,10 @@ PROTOTYPES = {
     "gops_b200_dsact_sample_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_float,
                                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_float,
                                                   C.c_void_p, C.c_void_p]),
+    "gops_b200_sac_losses": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_float,
+                                       C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p]),
     "gops_b200_peer_create": (C.c_int, [C.c_int32, C.c_int32, C.c_int64, C.POINTER(C.c_void_p)]),
     "gops_b200_peer_destroy": (C.c_int, [C.c_void_p]),
     "gops_b200_peer_region_bytes": (C.c_int, [C.c_void_p, C.POINTER(C.c_int64)]),

@@ -29,7 +29,7 @@ import torch.nn as nn
 from gops_b200 import _lib
 from gops_b200.algorithm.base import AlgorithmBase, ApprBase
 from gops_b200.create_pkg.create_apprfunc import create_apprfunc
-from gops_b200.ops.layerwise_mlp import LayerwiseMlpPair
+from gops_b200.ops.layerwise_mlp import layerwise_pair
 from gops_b200.utils.common_utils import get_apprfunc_dict
 from gops_b200.utils.flat_params import FusedAdam, ScalarAdam, polyak_update
 from gops_b200.utils.tensorboard_setup import tb_tags
@@ -64,15 +64,6 @@ class ApproxContainer(ApprBase):
 
     def create_action_distributions(self, logits):
         return self.policy.get_act_dist(logits)
-
-
-def _pair(a, b, max_batch: int, slots: int, tag: str) -> LayerwiseMlpPair:
-    """The library handles of two networks of identical shape, sized alike so that they can run as a pair."""
-    na, nb = a.layerwise(max_batch, slots, tag), b.layerwise(max_batch, slots, tag)
-    if (na.max_batch, na.slots) != (nb.max_batch, nb.slots):
-        mb, sl = max(na.max_batch, nb.max_batch), max(na.slots, nb.slots)
-        na, nb = a.layerwise(mb, sl, tag), b.layerwise(mb, sl, tag)
-    return LayerwiseMlpPair(na, nb)
 
 
 class DSACT(AlgorithmBase):
@@ -206,8 +197,8 @@ class DSACT(AlgorithmBase):
         pol, polT = nets.policy, nets.policy_target
         n_pol = pol.layerwise(B, 1, "train")
         n_polT = polT.layerwise(B, 1, "infer")
-        n_q = _pair(nets.q1, nets.q2, B, 2, "train")
-        n_qT = _pair(nets.q1_target, nets.q2_target, B, 1, "infer")
+        n_q = layerwise_pair(nets.q1, nets.q2, B, 2, "train")
+        n_qT = layerwise_pair(nets.q1_target, nets.q2_target, B, 1, "infer")
         for net, mod in ((n_pol, pol), (n_polT, polT), (n_q.a, nets.q1), (n_q.b, nets.q2), (n_qT.a, nets.q1_target),
                          (n_qT.b, nets.q2_target)):
             net.pack(mod.flat_params.sync())

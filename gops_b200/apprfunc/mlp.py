@@ -2,11 +2,12 @@
 
 Same constructor kwargs, class names, `state_dict` keys and init as the reference
 (gops/apprfunc/mlp.py: mlp() :36-41, DetermPolicy :50-77, FiniteHorizonPolicy :80-111,
-StateValue :309-329); `forward` runs the fused sm_90a inference kernels
+ActionValue :224-245, StateValue :309-329); `forward` runs the fused sm_90a inference kernels
 (`gops_b200_mlp_forward`) instead of nn.Sequential.  Training never calls `forward`: the
 algorithms hand the flat parameter vector to the fused rollout kernel.
 """
-__all__ = ["DetermPolicy", "FiniteHorizonPolicy", "FiniteHorizonFullPolicy", "StochaPolicy", "ActionValueDistri", "StateValue"]
+__all__ = ["DetermPolicy", "FiniteHorizonPolicy", "FiniteHorizonFullPolicy", "StochaPolicy", "ActionValue", "ActionValueDistri",
+           "StateValue"]
 
 import ctypes as C
 
@@ -235,6 +236,25 @@ class StochaPolicy(_LayerwiseNet, Action_Distribution):
         mean, log_std = torch.chunk(logits, chunks=2, dim=-1)
         std = torch.clamp(log_std, self.min_log_std, self.max_log_std).exp()       # 2 elementwise ops, inference only
         return torch.cat((mean, std), dim=-1).to(src)
+
+
+class ActionValue(_LayerwiseNet, Action_Distribution):
+    """Action value: (obs, act) -> q (reference mlp.py:224-245), the critic of SAC."""
+
+    _attr = "q"
+
+    def __init__(self, **kwargs):
+        super().__init__()
+        self._obs_dim, self.act_dim = kwargs["obs_dim"], kwargs["act_dim"]
+        self._build_net([self._obs_dim + self.act_dim] + list(kwargs["hidden_sizes"]) + [1], kwargs["hidden_activation"],
+                        kwargs.get("output_activation", "linear"))
+        self.action_distribution_cls = kwargs["action_distribution_cls"]
+
+    def forward(self, obs, act):
+        src = obs.device
+        flat = self.flat_params.sync()
+        x = torch.cat([obs, act], dim=-1).detach().to(flat.device, torch.float32).contiguous()
+        return torch.squeeze(self._raw(x), -1).to(src)
 
 
 class ActionValueDistri(_LayerwiseNet):

@@ -1,5 +1,6 @@
-// Device helpers shared by the DSAC (dsac.cu) and DSAC-T (dsact.cu) elementwise kernels: the ActionValueDistri head,
-// fixed-order block reductions and the gradient of the reparameterised tanh-Gaussian sample.
+// Device helpers shared by the DSAC (dsac.cu), DSAC-T (dsact.cu) and SAC (sac.cu) elementwise kernels: the
+// ActionValueDistri head, fixed-order block reductions, the soft TD target, the twin-min gradient and the gradient of
+// the reparameterised tanh-Gaussian sample.
 #pragma once
 #include <cuda_runtime.h>
 #include <math.h>
@@ -34,6 +35,18 @@ __device__ float block_reduce(long long B, float init, F f, Op op) {
 template <class F>
 __device__ float block_sum(long long B, F f) {
   return block_reduce(B, 0.f, f, [](float a, float b) { return a + b; });
+}
+
+// r + (1 - d) gamma (q - alpha logp), in the reference's operation order
+__device__ __forceinline__ float td_target(float r, float d, float gamma, float q, float alpha, float logp) {
+  return __fadd_rn(r, __fmul_rn(__fmul_rn(__fsub_rn(1.f, d), gamma), __fsub_rn(q, __fmul_rn(alpha, logp))));
+}
+
+// Gradient g of min(a, b) split as torch.minimum's backward does: all of it to the smaller value, half to each on a
+// tie, zero to the larger.
+__device__ __forceinline__ void twin_min_grad(float a, float b, float g, float& ga, float& gb) {
+  ga = a < b ? g : a == b ? 0.5f * g : 0.f;
+  gb = b < a ? g : a == b ? 0.5f * g : 0.f;
 }
 
 // d loss / d logits of one sample of the policy net, given dA(j) = d loss / d act_j and the coefficient c of log p in

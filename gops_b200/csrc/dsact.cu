@@ -22,11 +22,6 @@ using namespace gops::dsac;
 
 constexpr float kBias = 0.1f;                    // dsact.py:286
 
-// r + (1 - d) gamma (q - alpha logp), in the reference's operation order
-__device__ __forceinline__ float td_target(float r, float d, float gamma, float q, float alpha, float logp) {
-  return __fadd_rn(r, __fmul_rn(__fmul_rn(__fsub_rn(1.f, d), gamma), __fsub_rn(q, __fmul_rn(alpha, logp))));
-}
-
 // Twin critic loss (dsact.py:229-313).  q1o / q2o: critic outputs [B][2] (mean | raw std) at (obs, act); t1o / t2o:
 // target-critic outputs at (obs2, act2); z1 / z2: standard-normal noise of the two target samples.
 //   std_i = softplus(raw_i);  m_i = mean(std_i);  mean_std_i = (1 - tau_b) mean_std_i + tau_b m_i, or m_i if unset
@@ -109,8 +104,8 @@ __global__ void dsact_policy_loss_kernel(const float* __restrict__ q1o, const fl
   const float invB = 1.f / (float)B;
   const float l = block_sum(B, [&](long long i) {
     const float a = q1o[2 * i], b = q2o[2 * i];
-    const float g1 = a < b ? -invB : a == b ? -0.5f * invB : 0.f;
-    const float g2 = b < a ? -invB : a == b ? -0.5f * invB : 0.f;
+    float g1, g2;
+    twin_min_grad(a, b, -invB, g1, g2);
     dq1[2 * i] = g1; dq1[2 * i + 1] = 0.f;
     dq2[2 * i] = g2; dq2[2 * i + 1] = 0.f;
     return alpha * logp[i] - fminf(a, b);

@@ -95,3 +95,13 @@ class LayerwiseMlpPair:
                 _lib.ptr(grad_b), int(accumulate), _lib.ptr(dx_a), _lib.ptr(dx_b),
                 dx_a.stride(0) if dx_a is not None else 0, _lib.stream_ptr()))
         return dx_a, dx_b
+
+
+def layerwise_pair(a, b, max_batch: int, slots: int, tag: str) -> LayerwiseMlpPair:
+    """The library handles of two `_LayerwiseNet` modules of identical shape (twin critics), sized alike so that they
+    can run as a pair."""
+    na, nb = a.layerwise(max_batch, slots, tag), b.layerwise(max_batch, slots, tag)
+    if (na.max_batch, na.slots) != (nb.max_batch, nb.slots):
+        mb, sl = max(na.max_batch, nb.max_batch), max(na.slots, nb.slots)
+        na, nb = a.layerwise(mb, sl, tag), b.layerwise(mb, sl, tag)
+    return LayerwiseMlpPair(na, nb)

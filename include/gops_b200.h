@@ -351,6 +351,22 @@ int gops_b200_dsact_sample_backward(const float* logits, const float* eps, int64
                                     const float* d_act_2, int32_t ldda, int32_t act_col0, float logp_coeff,
                                     float* d_logits, void* stream);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * SAC (gops/algorithm/sac.py:159-241): every loss of one update in one launch, after three paired forwards of the
+ * twin ActionValue critics ([B] outputs each) with the pre-update weights: q1_out / q2_out at (obs, act), q1_new_out /
+ * q2_new_out at (obs, new_act), q1_next_out / q2_next_out (target critics) at (obs2, next_act).
+ *   y = rew + (1 - done) gamma (min(q1', q2') - alpha logp_next);  d_q{1,2}_out = 2 (q_i - y) / B
+ *   actor mean(alpha logp_new - min(q1, q2)) at new_act: d_q{1,2}_new_out = -1/B to the smaller critic, -1/(2B) to
+ *   each on a tie, 0 to the other
+ *   out6 = {loss_q1 + loss_q2, mean q1, mean q2, actor loss, entropy -mean(logp_new),
+ *           d loss_alpha / d log_alpha = -mean(logp_new + target_entropy)}
+ * The action gradient through both critics is gops_b200_dsact_sample_backward with logp_coeff alpha / B. */
+int gops_b200_sac_losses(const float* q1_out, const float* q2_out, const float* q1_new_out, const float* q2_new_out,
+                         const float* q1_next_out, const float* q2_next_out, const float* logp_new,
+                         const float* logp_next, const float* rew, const float* done, int64_t batch, float gamma,
+                         float alpha, float target_entropy, float* d_q1_out, float* d_q2_out, float* d_q1_new_out,
+                         float* d_q2_new_out, float* out6, void* stream);
+
 /* ---- data-parallel gradient exchange over NVLink peer memory, fused with Adam (peer.cu) ---------------------------
  * Replaces the gradient hand-over between replicas of the reference's synchronous trainer
  * (gops/trainer/off_sync_trainer.py:97-120: workers' get_remote_update_info -> remote_update with the averaged
