@@ -3,6 +3,7 @@ plus the shared plumbing of the fused ADP algorithms: plan creation, batch marsh
 NCCL all-reduce of the flat gradient, and the fused Adam step."""
 import ctypes as C
 from abc import ABC, ABCMeta, abstractmethod
+from copy import deepcopy
 from typing import Dict, Optional, Tuple
 
 import torch
@@ -28,6 +29,15 @@ class ApprBase(ABC, torch.nn.Module):
         for key in [k for k in kwargs if k.endswith("_scheduler")]:
             self.scheduler_dict[key] = getattr(torch.optim.lr_scheduler, kwargs[key]["name"])(
                 self.optimizer_dict[key.replace("_scheduler", "")], **kwargs[key]["params"])
+
+
+def target_copy(net: torch.nn.Module) -> torch.nn.Module:
+    """A Polyak target of `net`: a deep copy whose parameters take no gradient.  Made before the first update, the copy
+    owns its own `FlatParams` (bound to the copied module) and library handles."""
+    target = deepcopy(net)
+    for p in target.parameters():
+        p.requires_grad = False
+    return target
 
 
 class AlgorithmBase(metaclass=ABCMeta):
@@ -81,6 +91,16 @@ class AlgorithmBase(metaclass=ABCMeta):
 
     def to(self, device):
         self.networks.to(device)
+
+    def _device(self) -> torch.device:
+        """The networks' device; networks still on the CPU are moved to CUDA first (the updates run there only)."""
+        p = next(self.networks.parameters())
+        if not p.is_cuda:
+            if not torch.cuda.is_available():
+                raise RuntimeError(f"gops_b200: no CUDA device -- the {type(self).__name__} update has no CPU fallback")
+            self.networks.cuda()
+            p = next(self.networks.parameters())
+        return p.device
 
     def train(self):
         self.networks.train()
@@ -160,21 +180,12 @@ def allreduce_flat(gbuf: torch.Tensor, optimizer=None) -> bool:
 
 
 class FusedADPMixin:
-    """Shared by FHADP / INFADP: device handling, plans cache, fused rollout-gradient call."""
+    """Shared by FHADP / INFADP: plans cache, fused rollout-gradient call."""
 
     def _init_fused(self):
         self._plans: Dict[tuple, RolloutPlan] = {}
         if torch.cuda.is_available():
             self.networks.cuda()
-
-    def _device(self) -> torch.device:
-        p = next(self.networks.parameters())
-        if not p.is_cuda:
-            if not torch.cuda.is_available():
-                raise RuntimeError("gops_b200: no CUDA device -- the fused ADP update has no CPU fallback")
-            self.networks.cuda()
-            p = next(self.networks.parameters())
-        return p.device
 
     kernel_path = "auto"     # 'auto' | 'mma' | 'tc' (RolloutPlan.set_path); tests state and assert the path here
     MAX_PLANS = 4            # LRU: annealing pre_horizon must not leak one tape + blobs per distinct value
@@ -203,16 +214,19 @@ class FusedADPMixin:
     #                 step ahead of the device and no launch gap is exposed (bench.py states which mode it times).
     loss_lag = 0
 
-    def _tail_to_host(self, tail: torch.Tensor):
+    def _tail_to_host(self, *tails: torch.Tensor):
+        """The device tails of one update, side by side in one pinned buffer, as a host list (honours loss_lag)."""
         ring = self.__dict__.get("_tail_ring")
-        if ring is None or ring[0][0].device != torch.device("cpu"):
-            ring = [(torch.zeros(GRAD_TAIL, dtype=torch.float32).pin_memory(), torch.cuda.Event()) for _ in range(2)]
+        if ring is None:
+            ring = [(torch.zeros(len(tails) * GRAD_TAIL, dtype=torch.float32).pin_memory(), torch.cuda.Event())
+                    for _ in range(2)]
             self.__dict__["_tail_ring"] = ring
             self.__dict__["_tail_n"] = 0
         n = self.__dict__["_tail_n"]
         buf, ev = ring[n % 2]
-        with torch.cuda.device(tail.device):
-            buf.copy_(tail, non_blocking=True)
+        with torch.cuda.device(tails[0].device):
+            for i, tail in enumerate(tails):
+                buf[i * GRAD_TAIL:(i + 1) * GRAD_TAIL].copy_(tail, non_blocking=True)
             ev.record()
         self.__dict__["_tail_n"] = n + 1
         if self.loss_lag and n > 0:

@@ -8,13 +8,12 @@ Adam step plus a fused Polyak kernel."""
 __all__ = ["INFADP"]
 
 import time
-from copy import deepcopy
 from typing import Tuple
 
 import torch
 
 from gops_b200 import _lib
-from gops_b200.algorithm.base import AlgorithmBase, ApprBase, FusedADPMixin
+from gops_b200.algorithm.base import AlgorithmBase, ApprBase, FusedADPMixin, target_copy
 from gops_b200.create_pkg.create_apprfunc import create_apprfunc
 from gops_b200.create_pkg.create_env_model import create_env_model
 from gops_b200.utils.common_utils import get_apprfunc_dict
@@ -31,12 +30,8 @@ class ApproxContainer(ApprBase):
         policy_args = get_apprfunc_dict("policy", **kwargs)
         self.v = create_apprfunc(**v_args)
         self.policy = create_apprfunc(**policy_args)
-        self.v_target = deepcopy(self.v)
-        self.policy_target = deepcopy(self.policy)
-        for p in self.v_target.parameters():
-            p.requires_grad = False
-        for p in self.policy_target.parameters():
-            p.requires_grad = False
+        self.v_target = target_copy(self.v)
+        self.policy_target = target_copy(self.policy)
         self.policy_optimizer = FusedAdam(self.policy.flat_params, lr=kwargs["policy_learning_rate"])
         self.v_optimizer = FusedAdam(self.v.flat_params, lr=kwargs["value_learning_rate"])
         self.net_dict = {"v": self.v, "policy": self.policy}

@@ -17,47 +17,19 @@ identical multipliers (the reference's Ray replicas each run a controller of the
 __all__ = ["SPIL"]
 
 import time
-from copy import deepcopy
 from typing import Any, Tuple
 
 import numpy as np
 import torch
 
 from gops_b200 import _lib
-from gops_b200.algorithm.base import AlgorithmBase, ApprBase, FusedADPMixin
-from gops_b200.create_pkg.create_apprfunc import create_apprfunc
+from gops_b200.algorithm.base import AlgorithmBase, FusedADPMixin
+from gops_b200.algorithm.infadp import ApproxContainer   # noqa: F401  (ApproxContainer: registry contract)
 from gops_b200.create_pkg.create_env_model import create_env_model
-from gops_b200.utils.common_utils import get_apprfunc_dict
-from gops_b200.utils.flat_params import GRAD_TAIL, FusedAdam, polyak_update
+from gops_b200.utils.flat_params import GRAD_TAIL, polyak_update
 from gops_b200.utils.tensorboard_setup import tb_tags
 
 MODE_SPIL = 4        # gops_b200_plan_set_constraint mode
-
-
-class ApproxContainer(ApprBase):
-    """v, policy and their Polyak targets + one fused Adam per trained network (spil.py:32-70)."""
-
-    def __init__(self, **kwargs):
-        super().__init__(**kwargs)
-        v_args = get_apprfunc_dict("value", **kwargs)
-        policy_args = get_apprfunc_dict("policy", **kwargs)
-        self.v = create_apprfunc(**v_args)
-        self.policy = create_apprfunc(**policy_args)
-        self.v_target = deepcopy(self.v)
-        self.policy_target = deepcopy(self.policy)
-        for p in self.v_target.parameters():
-            p.requires_grad = False
-        for p in self.policy_target.parameters():
-            p.requires_grad = False
-        self.policy_optimizer = FusedAdam(self.policy.flat_params, lr=kwargs["policy_learning_rate"])
-        self.v_optimizer = FusedAdam(self.v.flat_params, lr=kwargs["value_learning_rate"])
-        self.net_dict = {"v": self.v, "policy": self.policy}
-        self.target_net_dict = {"v": self.v_target, "policy": self.policy_target}
-        self.optimizer_dict = {"v": self.v_optimizer, "policy": self.policy_optimizer}
-        self.scheduler_dict = {}
-
-    def create_action_distributions(self, logits):
-        return self.policy.get_act_dist(logits)
 
 
 class SPIL(AlgorithmBase, FusedADPMixin):
@@ -180,21 +152,7 @@ class SPIL(AlgorithmBase, FusedADPMixin):
 
     def _publish(self, tail_v: torch.Tensor, tail_p: torch.Tensor, start_time: float):
         """The update's one host read (honours loss_lag): both passes' tails in one pinned buffer."""
-        ring = self.__dict__.get("_spil_ring")
-        if ring is None:
-            ring = [(torch.zeros(2 * GRAD_TAIL, dtype=torch.float32).pin_memory(), torch.cuda.Event()) for _ in range(2)]
-            self.__dict__["_spil_ring"], self.__dict__["_spil_n"] = ring, 0
-        n = self.__dict__["_spil_n"]
-        buf, ev = ring[n % 2]
-        with torch.cuda.device(tail_v.device):
-            buf[:GRAD_TAIL].copy_(tail_v, non_blocking=True)
-            buf[GRAD_TAIL:].copy_(tail_p, non_blocking=True)
-            ev.record()
-        self.__dict__["_spil_n"] = n + 1
-        if self.loss_lag and n > 0:
-            buf, ev = ring[(n - 1) % 2]
-        ev.synchronize()
-        host = buf.tolist()
+        host = self._tail_to_host(tail_v, tail_p)
         self.tb_info[tb_tags["loss_critic"]] = host[0]
         self.tb_info[tb_tags["critic_avg_value"]] = host[1]
         self.tb_info[tb_tags["loss_actor"]] = host[GRAD_TAIL]

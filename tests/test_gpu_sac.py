@@ -18,7 +18,8 @@ import torch
 
 from golden_util import load, rel_l2
 from oracle import ref_shim, sac_ref
-from test_gpu_dsact import _check_weights
+from test_gpu_dsac import _kwargs as dsac_kwargs
+from test_gpu_dsact import _check_weights, _kwargs as dsact_kwargs
 
 pytestmark = pytest.mark.gpu
 needs_reference = pytest.mark.skipif(not ref_shim.available(), reason="reference tree not reachable")
@@ -193,8 +194,21 @@ def test_register_binding_and_three_trainer_steps():
 
 
 # ------------------------------------------------------------------------------------------------ (e) plugin surface
-def test_remote_update_equals_local_update():
-    kw = sac_ref.kwargs()
+# the soft actor-critic family shares its plugin surface: algorithm -> (kwargs, noise keys, critic gradient keys,
+# adjustable parameters)
+REMOTE = {
+    "SAC": (sac_ref.kwargs, ("eps_new", "eps_next"), ["q1_grad", "q2_grad"],
+            ("gamma", "tau", "auto_alpha", "alpha", "target_entropy")),
+    "DSAC": (lambda **over: dict(dsac_kwargs((64, 64, 64)), **over), ("eps_new", "eps_next", "z_next"), ["q_grad"],
+             ("gamma", "tau", "auto_alpha", "alpha", "bound", "delay_update")),
+    "DSACT": (lambda **over: dict(dsact_kwargs((64, 64, 64)), **over), ("eps_new", "eps_next", "z1_next", "z2_next"),
+              ["q1_grad", "q2_grad"], ("gamma", "tau", "auto_alpha", "alpha", "delay_update")),
+}
+
+
+def _remote_update_equals_local_update(name):
+    make_kw, noise_keys, grad_keys, adjustable = REMOTE[name]
+    kw = make_kw()
     torch.manual_seed(7)
     a = _create(kw)
     b = _create(kw)
@@ -204,22 +218,36 @@ def test_remote_update_equals_local_update():
     obs = torch.randn(B, 6, generator=g) * 0.3
     data = {"obs": obs.cuda(), "act": (torch.rand(B, 1, generator=g) * 2 - 1).cuda(), "rew": torch.randn(B, generator=g).cuda(),
             "obs2": (obs + 0.05 * torch.randn(B, 6, generator=g)).cuda(), "done": torch.zeros(B).cuda()}
-    for it in range(2):
-        noise = {"eps_new": torch.randn(B, 1, generator=g), "eps_next": torch.randn(B, 1, generator=g)}
+    tbs = []
+    for it in range(2):           # DSAC / DSAC-T (delay_update = 2): with and without the policy's step
+        noise = {k: torch.randn(B, 1, generator=g) if k.startswith("eps") else torch.randn(B, generator=g)
+                 for k in noise_keys}
         a.noise_override = b.noise_override = noise
         tb_a = a.local_update(data, it)
         tb_b, info = b.get_remote_update_info(data, it)
-        assert sorted(info) == ["iteration", "log_alpha_grad", "policy_grad", "q1_grad", "q2_grad"]
+        assert sorted(info) == sorted(["iteration", "log_alpha_grad", "policy_grad"] + grad_keys)
         b.remote_update(info)
-        assert all(tb_a[k] == tb_b[k] for k in TAGS)
+        tbs.append((tb_a, tb_b))
+        assert set(tb_a) == set(tb_b) and all(tb_a[k] == tb_b[k] for k in tb_a if k != "Time/Algorithm time [ms]-RL iter")
     sa, sb = a.state_dict(), b.state_dict()
     for k in sa:
         assert torch.equal(sa[k], sb[k]), k
-    c = _create(sac_ref.kwargs(auto_alpha=False))
+    c = _create(make_kw(auto_alpha=False))
     _, info = c.get_remote_update_info(data, 0)
     assert "log_alpha_grad" not in info
-    assert c.adjustable_parameters == ("gamma", "tau", "auto_alpha", "alpha", "target_entropy")
+    assert c.adjustable_parameters == adjustable
     assert c.target_entropy == -1
+    return tbs
+
+
+def test_remote_update_equals_local_update():
+    for tb_a, tb_b in _remote_update_equals_local_update("SAC"):
+        assert all(tb_a[k] == tb_b[k] for k in TAGS)
+
+
+@pytest.mark.parametrize("name", ["DSAC", "DSACT"])
+def test_remote_update_equals_local_update_distributional(name):
+    _remote_update_equals_local_update(name)
 
 
 def test_sac_runs_without_injected_noise():
