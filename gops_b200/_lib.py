@@ -10,7 +10,7 @@ MAX_ACT = 4
 MAX_LQ_N = 8
 
 ALG_FHADP, ALG_INFADP_POLICY, ALG_INFADP_VALUE = 0, 1, 2
-MODEL_IDPENDULUM, MODEL_LQ, MODEL_VEH3DOFCONTI, MODEL_VEH3DOF_TRACKING = 0, 1, 2, 3
+MODEL_IDPENDULUM, MODEL_LQ, MODEL_VEH3DOFCONTI, MODEL_VEH3DOF_TRACKING, MODEL_MOBILEROBOT = 0, 1, 2, 3, 4
 PATH_AUTO, PATH_MMA, PATH_TC = 0, 1, 2
 PATH_NAMES = {0: "none", 1: "mma", 2: "tc"}
 ACT_IDS = {"relu": 0, "elu": 1, "gelu": 2, "selu": 3, "sigmoid": 4, "tanh": 5, "linear": 6}
@@ -75,6 +75,7 @@ PROTOTYPES = {
     "gops_b200_plan_last_path": (C.c_int, [C.c_void_p]),
     "gops_b200_plan_set_constraint": (C.c_int, [C.c_void_p, C.c_int, C.c_float]),
     "gops_b200_plan_set_spil_weights": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "gops_b200_plan_set_model_io": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "gops_b200_spil_controller": (C.c_int, [C.c_void_p, C.c_int64, C.c_double, C.c_double, C.c_double, C.c_double,
                                             C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gops_b200_plan_param_count": (C.c_int64, [C.c_void_p, C.c_int]),

@@ -9,6 +9,7 @@ namespace gops {
 
 constexpr int MAXA = GOPS_B200_MAX_ACT;
 constexpr int LQN = GOPS_B200_MAX_LQ_N;
+constexpr int kMaxObs = 16;     // observation entries with ClipObservation bounds (state==obs models: pyth_mobilerobot has 13)
 
 // ---------------------------------------------------------------------------------------------
 // mbarrier + TMA (cp.async.bulk) primitives: weights are staged global -> shared by the bulk-copy

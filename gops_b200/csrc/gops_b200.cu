@@ -106,10 +106,18 @@ const ModelKernels* kernels_of(int model) {
     case GOPS_MODEL_LQ: return &kernels_lq();
     case GOPS_MODEL_VEH3DOFCONTI: return &kernels_vehconti();
     case GOPS_MODEL_VEH3DOF_TRACKING: return &kernels_vehtrack();
+    case GOPS_MODEL_MOBILEROBOT: return &kernels_mobilerobot();
     default: return nullptr;
   }
 }
-int model_ns(int model) { return model == GOPS_MODEL_LQ ? LQN : (model == GOPS_MODEL_VEH3DOFCONTI ? 7 : 6); }
+int model_ns(int model) {
+  switch (model) {
+    case GOPS_MODEL_LQ: return LQN;
+    case GOPS_MODEL_VEH3DOFCONTI: return ModelVehConti::NS;
+    case GOPS_MODEL_MOBILEROBOT: return ModelMobileRobot::NS;
+    default: return 6;
+  }
+}
 
 }  // namespace
 
@@ -225,6 +233,8 @@ int check_batch(const gops_b200_plan* pl, const gops_b200_batch* b, bool layerwi
     if (layerwise && pl->desc.veh_detour && (!b->surr || b->ref_t + pl->kp.horizon + 1 > b->surr_len))
       return fail("veh3dof_tracking_detour needs the surrounding-vehicle predictions (ContextState.constraint), t + horizon + 1 points");
   }
+  if (pl->desc.model == GOPS_MODEL_MOBILEROBOT && !pl->kp.noise)
+    return fail("pyth_mobilerobot needs its obstacle noise [horizon][batch][2] (gops_b200_plan_set_model_io)");
   return 0;
 }
 
@@ -592,6 +602,12 @@ int plan_constants(const gops_b200_plan_desc* d, KParams& kp) {
       if (!(d->veh_length > d->veh_width) || !(d->veh_width > 0.f)) return fail("veh3dof_tracking_detour: need veh_length > veh_width > 0");
     }
   }
+  if (d->model == GOPS_MODEL_MOBILEROBOT) {
+    obs_dim_model = ModelMobileRobot::NS;
+    if (act_dim != 2) return fail("pyth_mobilerobot has 2 actions");
+    // the noise is drawn once per model step: a repeated step would need draws per repetition
+    if (d->repeat_num > 1) return fail("repeat_num > 1 (ActionRepeat) is not built for pyth_mobilerobot");
+  }
   if (d->policy.in_dim != obs_dim_model) return fail("policy in_dim does not match the env model obs_dim");
   if (d->model == GOPS_MODEL_IDPENDULUM && act_dim != 1) return fail("idpendulum has 1 action");
 
@@ -606,7 +622,7 @@ int plan_constants(const gops_b200_plan_desc* d, KParams& kp) {
   kp.action_scale = d->action_scale; kp.clip_action = d->clip_action; kp.mask_at_done = d->mask_at_done;
   kp.reward_shaping = d->reward_shaping; kp.reward_shift = d->reward_shift; kp.reward_scale = d->reward_scale;
   kp.obs_scaling = d->obs_scaling ? 1 : 0;
-  kp.repeat_num = d->repeat_num > 0 ? d->repeat_num : 0;
+  kp.repeat_num = (d->repeat_num > 0 && d->model != GOPS_MODEL_MOBILEROBOT) ? d->repeat_num : 0;
   kp.sum_reward = d->sum_reward ? 1 : 0;
   if (kp.repeat_num > 0 && !(d->model == GOPS_MODEL_IDPENDULUM || d->model == GOPS_MODEL_LQ))
     return fail("repeat_num (ActionRepeat) is supported for state==obs models only (not built for vehicle models)");
@@ -621,9 +637,11 @@ int plan_constants(const gops_b200_plan_desc* d, KParams& kp) {
     kp.pol_mid[j] = (d->pol_act_high[j] + d->pol_act_low[j]) / 2.f;
   }
   const bool state_is_obs = d->model == GOPS_MODEL_IDPENDULUM || d->model == GOPS_MODEL_LQ;
-  for (int f = 0; f < LQN; ++f) {
-    kp.obs_low[f] = (state_is_obs && f < obs_dim_model) ? d->obs_low[f] : -INFINITY;
-    kp.obs_high[f] = (state_is_obs && f < obs_dim_model) ? d->obs_high[f] : INFINITY;
+  const bool robot = d->model == GOPS_MODEL_MOBILEROBOT;   // 13 bounds: the model's own (the descriptor carries 8)
+  for (int f = 0; f < kMaxObs; ++f) {
+    const bool in = f < obs_dim_model;
+    kp.obs_low[f] = (robot && in) ? kRobotObsLow[f] : (state_is_obs && in && f < LQN) ? d->obs_low[f] : -INFINITY;
+    kp.obs_high[f] = (robot && in) ? kRobotObsHigh[f] : (state_is_obs && in && f < LQN) ? d->obs_high[f] : INFINITY;
     if (isfinite(kp.obs_low[f]) || isfinite(kp.obs_high[f])) finite_obs_bound = true;
   }
   kp.clip_obs = (d->clip_obs && finite_obs_bound) ? 1 : 0;   // clipping to +-inf is the identity
@@ -884,8 +902,8 @@ int gops_b200_plan_set_constraint(gops_b200_plan* pl, int mode, float coef) {
   if (mode < 0 || mode > 4) return fail("unknown constraint mode");
   if (mode == 4) {
     // SPIL runs on the mma.sync / FFMA rollout kernel only
-    if (!(pl->desc.model == GOPS_MODEL_VEH3DOFCONTI && pl->desc.veh_errcstr))
-      return fail("the SPIL constraint mode is built for pyth_veh3dofconti_errcstr only");
+    if (!(pl->desc.model == GOPS_MODEL_VEH3DOFCONTI && pl->desc.veh_errcstr) && pl->desc.model != GOPS_MODEL_MOBILEROBOT)
+      return fail("the SPIL constraint mode is built for pyth_veh3dofconti_errcstr and pyth_mobilerobot only");
     if (pl->desc.alg != GOPS_ALG_FHADP && pl->desc.alg != GOPS_ALG_INFADP_VALUE)
       return fail("the SPIL constraint mode needs an FHADP (policy) or INFADP_VALUE (value) plan");
     if (pl->desc.open_loop || pl->tc_ok || layerwise_built(pl))
@@ -908,6 +926,14 @@ int gops_b200_plan_set_constraint(gops_b200_plan* pl, int mode, float coef) {
 int gops_b200_plan_set_spil_weights(gops_b200_plan* pl, const float* weights) {
   if (!pl) return fail("null plan");
   pl->kp.spil_w = weights;
+  return 0;
+}
+
+int gops_b200_plan_set_model_io(gops_b200_plan* pl, const float* noise, float* constraint_out) {
+  if (!pl) return fail("null plan");
+  if (pl->desc.model != GOPS_MODEL_MOBILEROBOT) return fail("plan_set_model_io: this env model takes no noise");
+  pl->kp.noise = noise;
+  pl->kp.cstr_out = constraint_out;
   return 0;
 }
 
@@ -1060,6 +1086,8 @@ int gops_b200_model_step(gops_b200_plan* pl, const gops_b200_batch* b, const flo
     ++g_launches;
     return launched("veh_step launch");
   }
+  if (pl->desc.model == GOPS_MODEL_MOBILEROBOT && !p.noise)
+    return fail("model_step: pyth_mobilerobot needs its obstacle noise [batch][2] (gops_b200_plan_set_model_io)");
   StepFn fn = kernels_of(pl->desc.model)->step;
   if (!fn) return fail("model_step: env model kind not built into this library");
   fn<<<grid, 128, 0, st>>>(p, action, act_dim, next_obs, reward, next_done);

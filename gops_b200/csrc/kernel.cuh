@@ -16,6 +16,21 @@ __device__ __forceinline__ float spil_phi(float c, float& dlog) {
   return (float)(1.0 + 0.07) / den;
 }
 
+// SPIL's per-sample constraint record of one step, constraints c[0, NC) (NC <= 2): the value pass keeps one safe-so-far
+// flag per constraint (traj_issafe *= constraint <= 0, spil.py:200, 207), the policy pass the running product of
+// Phi(constraint) (c_mul = c_mul * Phi(c), spil.py:240-252)
+template <int NC>
+__device__ __forceinline__ void spil_track(bool pev, const float* c, float& ca, float& cb) {
+  if (pev) {
+    ca = c[0] <= 0.f ? ca : 0.f;
+    if (NC > 1) cb = c[1] <= 0.f ? cb : 0.f;
+  } else {
+    float dl;
+    ca *= spil_phi(c[0], dl);
+    if (NC > 1) cb *= spil_phi(c[1], dl);
+  }
+}
+
 // One CTA = NT threads = NT samples per chunk; MLP GEMMs run over SUB = NT/S sub-tiles of S samples that
 // reuse one set of activation tiles; the per-sample dynamics (forward and adjoint) run on every thread.
 // HD = 64: weights (TMA-staged), weight-gradient accumulators and X live in shared memory.
@@ -156,11 +171,17 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
     float vacc = 0.f;
     // constrained variants: discounted exterior|linear sum, interior (log) sum; SPIL: per constraint the safe-so-far flag
     // (value pass) or the running product of Phi (policy pass)
-    float cacc_a = p.cstr_mode == 4 ? 1.f : 0.f, cacc_b = cacc_a;
+    // (one constraint: the second record stays 0, so scalar tail slot 3 reads 0)
+    float cacc_a = p.cstr_mode == 4 ? 1.f : 0.f, cacc_b = M::NC == 1 ? 0.f : cacc_a;
     bool infeasible = false;
     int path = 0, spd = 0;                       // vehicle models: reference path / speed profile ids
     RefWindow<M::KIND, NT> win;
     win.base = nullptr; win.k0 = 0;
+    // models with noise: this sample's draws of step k, [H][B][NZ]
+    auto noise_at = [&](int k) -> const float* {
+      if constexpr (M::KIND == 0 && M::NC > 0) return p.noise + ((size_t)k * B + gs) * M::NZ;
+      else return nullptr;
+    };
     if constexpr (M::KIND == 0) {
 #pragma unroll
       for (int f = 0; f < NS; ++f) st[f] = f < obs_dim ? t.X[f * XS + col] : 0.f;
@@ -220,16 +241,9 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
             bool inf;
 #pragma unroll
             for (int f = 0; f < 6; ++f) oc[f] = to_inner(p, f, t.X[f * XS + col]);
-            if (p.cstr_mode == 4) {
-              const float c0 = fabsf(oc[1]) - p.cstr_y_tol, c1 = fabsf(oc[3]) - p.cstr_u_tol;
-              if (alg == ALG_PEV) {          // traj_issafe *= constraint <= 0   (spil.py:200, 207)
-                cacc_a = c0 <= 0.f ? cacc_a : 0.f;
-                cacc_b = c1 <= 0.f ? cacc_b : 0.f;
-              } else {                       // c_mul = c_mul * Phi(constraint)  (spil.py:240-252)
-                float dl;
-                cacc_a *= spil_phi(c0, dl);
-                cacc_b *= spil_phi(c1, dl);
-              }
+            if (p.cstr_mode == 4) {            // the constraints of the INCOMING observation
+              const float cc[2] = {fabsf(oc[1]) - p.cstr_y_tol, fabsf(oc[3]) - p.cstr_u_tol};
+              spil_track<2>(alg == ALG_PEV, cc, cacc_a, cacc_b);
             } else {
               cstr_eval(oc, ce, cl, ci, inf);
               cacc_a += (p.cstr_mode == 2 ? cl : ce) * p.gpow[k];
@@ -241,10 +255,14 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
         if constexpr (M::KIND == 0) {
           // state==obs models: `st` is the wrapper-level (outer) observation
           if (valid) {
-            wrapped_step<M>(p, obs_dim, st, a, active, r, dn);
+            float c[nc_slots(M::NC)];
+            wrapped_step<M>(p, obs_dim, st, a, active, r, dn, noise_at(k), c);
 #pragma unroll
             for (int f = 0; f < NS; ++f)
               if (f < obs_dim) t.X[f * XS + col] = st[f];
+            if constexpr (M::NC > 0) {         // the constraints of the RAW next state, frozen (done) samples included
+              if (p.cstr_mode == 4) spil_track<M::NC>(alg == ALG_PEV, c, cacc_a, cacc_b);
+            }
           }
         } else if (active) {
           const VehC vc = veh_const();
@@ -311,7 +329,7 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
       stage(p.blob_vtg, V.blob);  // leading __syncthreads also publishes X = o_n
       const float gn = p.gpow[H];
       // SPIL's value target keeps gamma^n v_target(o_n) for done samples too (spil.py:209, no (~d) mask)
-      const bool term = valid && (!dn || (M::KIND == 1 && p.cstr_mode == 4));
+      const bool term = valid && (!dn || (M::NC > 0 && p.cstr_mode == 4));
       if (alg == ALG_PIM) {
         t.Z[col] = term ? -gn * p.inv_B : 0.f;     // row 0: d loss / d v_target(o_n); rows 1 (+5) receive v
         scope_sync();
@@ -343,7 +361,7 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
     }
 
     if (alg == ALG_PEV) {
-      if constexpr (M::KIND == 1) {
+      if constexpr (M::NC > 0) {
         if (p.cstr_mode == 4 && valid) {     // SPIL: safe trajectories per constraint -> scalar tail slots 2 and 3
           cint_acc += cacc_a;
           feas_acc += cacc_b;
@@ -375,11 +393,12 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
     }
 
     float ret = vacc;                    // the per-sample objective whose negated batch mean is the loss
-    if constexpr (M::KIND == 1) {
+    if constexpr (M::NC > 0) {
       if (p.cstr_mode == 4 && valid) {
         // SPIL: loss_pi = -mean(w_r R + sum_i w_c,i prod_k Phi(c_k,i))   (spil.py:253-255); tail [1] mean R,
         // [2] / [3] mean Phi product of constraint 0 / 1
-        ret = p.spil_w[0] * vacc + (cacc_a * p.spil_w[1] + cacc_b * p.spil_w[2]);
+        if constexpr (M::NC == 1) ret = p.spil_w[0] * vacc + cacc_a * p.spil_w[1];
+        else ret = p.spil_w[0] * vacc + (cacc_a * p.spil_w[1] + cacc_b * p.spil_w[2]);
         vmean_acc += vacc * p.inv_B;
         cint_acc += cacc_a * p.inv_B;
         feas_acc += cacc_b * p.inv_B;
@@ -445,6 +464,9 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
       }
       if (P.time_input) t.X[(P.in - 1) * XS + col] = (float)(k + 1);
       const bool active = valid && (p.mask_at_done ? !dnk : true);
+      // SPIL on a model whose constraints read the raw next state: a frozen (done) sample still steps, and its constraint
+      // pulls back onto the action and the frozen observation
+      const bool cstep = M::KIND == 0 && M::NC > 0 && p.cstr_mode == 4 && valid;
       float ro6[6];               // KIND 1: d loss / d obs_k[0..5] through the reward
 #pragma unroll
       for (int f = 0; f < 6; ++f) ro6[f] = 0.f;
@@ -452,19 +474,31 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
         float zb[MAXA];
 #pragma unroll
         for (int j = 0; j < MAXA; ++j) zb[j] = 0.f;
-        if (active) {
+        if (active || cstep) {
           float z[MAXA], a[MAXA], g[MAXA], abar[MAXA];
 #pragma unroll
           for (int j = 0; j < MAXA; ++j) z[j] = j < P.out ? tape[(k * TCH + NS + 1 + j) * NT + tid] : 0.f;
           process_action(p, P.out, z, a, g, nullptr);
           float rho = reward_adjoint(p, k);
-          if constexpr (M::KIND == 1) {
+          if constexpr (M::NC > 0) {
             if (p.cstr_mode == 4) rho *= p.spil_w[0];     // SPIL: w_r weights the return
           }
 #pragma unroll
           for (int j = 0; j < MAXA; ++j) abar[j] = 0.f;
           if constexpr (M::KIND == 0) {
-            wrapped_step_bwd<M>(p, obs_dim, st, a, rho, lam, abar);     // lam: adjoint of the outer observation obs_{k+1}
+            // lam: adjoint of the outer observation obs_{k+1}
+            if constexpr (M::NC > 0) {
+              // d(-w_c / B prod_s Phi(c_s)) / dc_k = -w_c / B (prod_s Phi_s) dlog Phi(c_k)   (see the KIND 1 term below)
+              const float wc = p.cstr_mode == 4 ? -p.spil_w[1] * p.inv_B * cacc_a : 0.f;
+              auto cbar_of = [wc](const float* c, float* cbar) {
+                float dl;
+                spil_phi(c[0], dl);
+                cbar[0] = wc * dl;
+              };
+              wrapped_step_bwd<M, MAXA, WrapRt, false>(p, obs_dim, st, a, rho, lam, abar, noise_at(k), active, cbar_of);
+            } else {
+              wrapped_step_bwd<M>(p, obs_dim, st, a, rho, lam, abar);
+            }
           } else {
             const VehC vc = veh_const();
             veh_step_bwd(vc, st, a, lam, abar);
@@ -525,7 +559,7 @@ __global__ void __launch_bounds__(NT, 1) rollout_kernel(const __grid_constant__ 
           }
         }
       }
-      if (active && k > 0) {
+      if ((active || cstep) && k > 0) {
         if constexpr (M::KIND == 0) {
 #pragma unroll
           for (int f = 0; f < NS; ++f)
@@ -668,8 +702,14 @@ __global__ void model_step_kernel(const __grid_constant__ KParams p, const float
     a[j] = j < act_dim ? wrap_action(p, j, action[gs * act_dim + j], gg) : 0.f;
   }
   bool dn = p.done[gs] != 0.f;
-  float r = 0.f;
-  wrapped_step<M>(p, obs_dim, st, a, !(p.mask_at_done && dn), r, dn);     // a masked sample stays done
+  float r = 0.f, c[nc_slots(M::NC)];
+  const float* nz = nullptr;
+  if constexpr (M::NC > 0) nz = p.noise + (size_t)gs * M::NZ;
+  wrapped_step<M>(p, obs_dim, st, a, !(p.mask_at_done && dn), r, dn, nz, c);     // a masked sample stays done
+  if constexpr (M::NC > 0) {
+    if (p.cstr_out)
+      for (int i = 0; i < M::NC; ++i) p.cstr_out[gs * M::NC + i] = c[i];
+  }
   r = shape_reward(p, r);
   for (int f = 0; f < obs_dim; ++f) next_obs[gs * obs_dim + f] = st[f];
   reward[gs] = r;

@@ -78,6 +78,7 @@ const ModelKernels& kernels_idp();
 const ModelKernels& kernels_lq();
 const ModelKernels& kernels_vehconti();
 const ModelKernels& kernels_vehtrack();
+const ModelKernels& kernels_mobilerobot();
 
 // veh3dof_tracking_detour (lw_detour.cuh, kernels_vehtrack.cu): forward / reverse step kernels of the layer-wise path
 // (init is the model's), the model step and the loss / constraint scalars

@@ -2,6 +2,7 @@
 #pragma once
 #include "rollout.cuh"
 #include "models_veh.cuh"
+#include "models_robot.cuh"
 
 namespace gops {
 
@@ -97,17 +98,50 @@ __device__ __forceinline__ float reward_adjoint(const KParams& p, int k) {
   return -p.gpow[k] * p.inv_B * (p.reward_shaping ? p.reward_scale : 1.f);
 }
 
+// The model step and its adjoint.  A model with constraints (NC > 0) also reads its noise nz and reports / receives the
+// constraints of the raw next state (c / cbar); the others take neither.
+template <class M>
+__device__ __forceinline__ void model_fwd(const KParams& p, float* s, const float* a, const float* nz, float& r, bool& d,
+                                          float* c) {
+  if constexpr (M::NC > 0) M::step(p, s, a, nz, r, d, c);
+  else M::step(p, s, a, r, d);
+}
+template <class M, bool UNROLL>
+__device__ __forceinline__ void model_bwd(const KParams& p, const float* s, const float* a, const float* nz, float rho,
+                                          float* lam, float* abar, const float* cbar) {
+  if constexpr (M::NC > 0) M::template step_bwd<UNROLL>(p, s, a, nz, rho, lam, abar, cbar);
+  else M::template step_bwd<UNROLL>(p, s, a, rho, lam, abar);
+}
+__host__ __device__ constexpr int nc_slots(int nc) { return nc > 0 ? nc : 1; }
+struct NoCstrAdjoint {       // models without constraints: nothing to differentiate
+  __device__ void operator()(const float*, float*) const {}
+};
+
 // One step of a state==obs model (KIND 0) inside its wrappers, on the outer observation st[0..obs_dim) (in place):
 // ScaleObservation -> ActionRepeat (the masked model step repeated with the same action) -> unscale -> ClipObservation.
 // When `active` (not frozen by MaskAtDone) r receives the raw reward and dn the new done flag; else both are left alone.
+// A model with constraints (no ActionRepeat) steps frozen samples too, as the reference's MaskAtDone does: c receives
+// the constraints of that raw step (info["constraint"] is not masked), the frozen observation stays.
 template <class M, class W = WrapRt>
 __device__ __forceinline__ void wrapped_step(const KParams& p, int obs_dim, float* st, const float* a, bool active,
-                                             float& r, bool& dn) {
+                                             float& r, bool& dn, const float* nz = nullptr, float* c = nullptr) {
   constexpr int NS = M::NS;
   float in[NS];
 #pragma unroll
   for (int f = 0; f < NS; ++f) in[f] = (W::obs_scaling(p) && f < obs_dim) ? st[f] / p.osc[f] - p.osh[f] : st[f];
-  if (active) {
+  if constexpr (M::NC > 0) {
+    float nx[NS], rj;
+    bool md;
+#pragma unroll
+    for (int f = 0; f < NS; ++f) nx[f] = in[f];
+    model_fwd<M>(p, nx, a, nz, rj, md, c);
+    if (active) {
+#pragma unroll
+      for (int f = 0; f < NS; ++f) in[f] = nx[f];
+      r = rj;
+      dn = md;
+    }
+  } else if (active) {
     bool md = false;
     const int reps = W::repeat_num(p) > 0 ? W::repeat_num(p) : 1;
     float rsum = 0.f, rj = 0.f;
@@ -126,29 +160,44 @@ __device__ __forceinline__ void wrapped_step(const KParams& p, int obs_dim, floa
   }
 }
 
-// Adjoint of wrapped_step for an active sample: st = outer observation before the step, lam = adjoint of the outer
-// observation after it (in) / before it (out), rho = dL/d(raw reward), abar[j] += dL/d a[j].  Chain of the step:
+// Adjoint of wrapped_step: st = outer observation before the step, lam = adjoint of the outer observation after it
+// (in) / before it (out), rho = dL/d(raw reward), abar[j] += dL/d a[j].  Chain of the step:
 //   obs_k -(1/scale, -shift)-> inner_0 -[model step x reps, same action]-> inner_reps -(+shift, *scale)-> clip -> obs_k+1
 // NA: length of abar (the kernel's action count; M reads a[0, NA) and writes at most MAXA adjoints).  UNROLL: passed to
-// M::step_bwd.
-template <class M, int NA = MAXA, class W = WrapRt, bool UNROLL = false>
+// M::step_bwd.  Models with constraints: cbar_of(c, cbar) turns the constraints of the raw step into their adjoints; a
+// frozen sample (!active) passes lam through unchanged and adds only what the constraints pull back.
+template <class M, int NA = MAXA, class W = WrapRt, bool UNROLL = false, class CB = NoCstrAdjoint>
 __device__ __forceinline__ void wrapped_step_bwd(const KParams& p, int obs_dim, const float* st, const float* a,
-                                                 float rho, float* lam, float* abar) {
+                                                 float rho, float* lam, float* abar, const float* nz = nullptr,
+                                                 bool active = true, CB cbar_of = CB()) {
   constexpr int NS = M::NS;
   const int reps = W::repeat_num(p) > 0 ? W::repeat_num(p) : 1;
-  float in0[NS], cur[NS];
+  float in0[NS], cur[NS], c[nc_slots(M::NC)], cbar[nc_slots(M::NC)], keep[NS];
 #pragma unroll
   for (int f = 0; f < NS; ++f) in0[f] = (W::obs_scaling(p) && f < obs_dim) ? st[f] / p.osc[f] - p.osh[f] : st[f];
-  if (W::clip_obs(p)) {            // clip passes gradient only where the raw next observation is inside
+  if constexpr (M::NC > 0) {
+    if (!active) {            // obs_k+1 = clip(obs_k): the adjoint passes where obs_k is inside the bounds
+#pragma unroll
+      for (int f = 0; f < NS; ++f) {
+        keep[f] = (W::clip_obs(p) && (st[f] < p.obs_low[f] || st[f] > p.obs_high[f])) ? 0.f : lam[f];
+        lam[f] = 0.f;
+      }
+      rho = 0.f;
+    }
+  }
+  if (W::clip_obs(p) || M::NC > 0) {   // the raw next state: clip passes gradient only where it is inside; constraints
     float rr;
     bool md;
 #pragma unroll
     for (int f = 0; f < NS; ++f) cur[f] = in0[f];
-    for (int j = 0; j < reps; ++j) M::step(p, cur, a, rr, md);
+    for (int j = 0; j < reps; ++j) model_fwd<M>(p, cur, a, nz, rr, md, c);
+    if constexpr (M::NC > 0) cbar_of(c, cbar);
+    if (W::clip_obs(p)) {
 #pragma unroll
-    for (int f = 0; f < NS; ++f) {
-      const float o = (W::obs_scaling(p) && f < obs_dim) ? (cur[f] + p.osh[f]) * p.osc[f] : cur[f];
-      if (o < p.obs_low[f] || o > p.obs_high[f]) lam[f] = 0.f;
+      for (int f = 0; f < NS; ++f) {
+        const float o = (W::obs_scaling(p) && f < obs_dim) ? (cur[f] + p.osh[f]) * p.osc[f] : cur[f];
+        if (o < p.obs_low[f] || o > p.obs_high[f]) lam[f] = 0.f;
+      }
     }
   }
   if (W::obs_scaling(p)) {
@@ -161,11 +210,11 @@ __device__ __forceinline__ void wrapped_step_bwd(const KParams& p, int obs_dim, 
     bool md;
 #pragma unroll
     for (int f = 0; f < NS; ++f) cur[f] = in0[f];
-    for (int q = 0; q < j; ++q) M::step(p, cur, a, rr, md);      // state before repeat j
+    for (int q = 0; q < j; ++q) model_fwd<M>(p, cur, a, nz, rr, md, c);      // state before repeat j
     const float rho_j = (W::repeat_num(p) == 0 || p.sum_reward || j == reps - 1) ? rho : 0.f;
 #pragma unroll
     for (int q = 0; q < MAXA; ++q) aj[q] = 0.f;
-    M::template step_bwd<UNROLL>(p, cur, a, rho_j, lam, aj);
+    model_bwd<M, UNROLL>(p, cur, a, nz, rho_j, lam, aj, cbar);
 #pragma unroll
     for (int q = 0; q < NA; ++q) abar[q] += aj[q];
   }
@@ -173,6 +222,12 @@ __device__ __forceinline__ void wrapped_step_bwd(const KParams& p, int obs_dim, 
 #pragma unroll
     for (int f = 0; f < NS; ++f)
       if (f < obs_dim) lam[f] /= p.osc[f];
+  }
+  if constexpr (M::NC > 0) {
+    if (!active) {
+#pragma unroll
+      for (int f = 0; f < NS; ++f) lam[f] += keep[f];
+    }
   }
 }
 
@@ -286,7 +341,7 @@ __device__ __forceinline__ void idp_substep_bwd(float v1, float v2, const IdpAux
 }
 
 struct ModelIdp {
-  static constexpr int NS = 6, KIND = 0;
+  static constexpr int NS = 6, KIND = 0, NC = 0;
   // forward: s <- next state; returns raw model reward and done   (:199-216, :126-172)
   __device__ static __forceinline__ void step(const KParams&, float* s, const float* a, float& rew, bool& done) {
     const IdpC c = idp_const();
@@ -340,7 +395,7 @@ struct ModelIdp {
 // pyth_lq   (env_ocp/resources/lq_base.py:89-141, :343-354)   zero-padded to LQN x MAXA
 // =============================================================================================
 struct ModelLq {
-  static constexpr int NS = LQN, KIND = 0;
+  static constexpr int NS = LQN, KIND = 0, NC = 0;
   __device__ static __forceinline__ void step(const KParams& p, float* s, const float* a, float& rew, bool& done) {
     float rs = 0.f, ra = 0.f, tmp[LQN];
 #pragma unroll
@@ -395,7 +450,7 @@ struct ModelLq {
 // KIND 2: env_gen_ocp veh3dof_tracking (window = slice of the caller's reference tensor)
 // =============================================================================================
 struct ModelVehConti {
-  static constexpr int NS = 7, KIND = 1;   // x, y, phi, u, v, w, ref_time
+  static constexpr int NS = 7, KIND = 1, NC = 2;   // x, y, phi, u, v, w, ref_time; NC: (|y_err|, |u_err|) constraints
   // reward from the INCOMING inner observation o (Veh3dofcontiModel.compute_reward :161-177)
   __device__ static __forceinline__ float reward(const float* o, const float* a) {
     return -(0.04f * (o[0] * o[0]) + 0.04f * (o[1] * o[1]) + 0.02f * (o[2] * o[2]) + 0.02f * (o[3] * o[3]) +
@@ -415,7 +470,7 @@ struct ModelVehConti {
   }
 };
 struct ModelVehTrack {
-  static constexpr int NS = 6, KIND = 2;
+  static constexpr int NS = 6, KIND = 2, NC = 0;
   // reward from the CURRENT state s against reference point q = reference[:, t] (veh3dof_tracking_model.py:59-73)
   __device__ static __forceinline__ float reward(const float* s, const float* q, const float* a) {
     const float ex = s[0] - q[0], ey = s[1] - q[1], ep = angle_normalize(s[2] - q[2]), eu = s[3] - q[3];

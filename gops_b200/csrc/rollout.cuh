@@ -90,6 +90,10 @@ struct KParams {
   int cstr_mode;
   float cstr_coef, cstr_y_tol, cstr_u_tol;
   const float* spil_w;     // cstr_mode 4, policy pass: device [w_r, w_c0, w_c1] written by the SPIL controller kernel
+  // models with noise (pyth_mobilerobot): device draws, [H][B][2] per rollout / [B][2] per model step; the model step's
+  // [B][NC] constraints out (gops_b200_plan_set_model_io)
+  const float* noise;
+  float* cstr_out;
   // env_gen_ocp veh3dof_tracking_detour (lw_detour.cuh): surrounding-vehicle predictions [B][surr_len][1][5] (x, y, phi, u,
   // delta), circle offset d = (length - width) / 2 and 2 r = width of the bicircle collision model
   int veh_detour, surr_len;
@@ -105,7 +109,7 @@ struct KParams {
   const float* osh;
   float min_action[MAXA], max_action[MAXA], act_low[MAXA], act_high[MAXA];
   float pol_half[MAXA], pol_mid[MAXA];
-  float obs_low[LQN], obs_high[LQN];
+  float obs_low[kMaxObs], obs_high[kMaxObs];   // ClipObservation bounds of the state==obs models
   // LQ
   int lq_n, lq_m;
   float lq_inv_IA[LQN * LQN], lq_B[LQN * MAXA], lq_Q[LQN], lq_R[MAXA];

@@ -119,10 +119,16 @@ def fused_forward(top, obs, action, done, info):
         rew = torch.empty(B, dtype=torch.float32, device=dev)
         ndone = torch.empty(B, dtype=torch.float32, device=dev)
         extra = base.alloc_next_info(B, dev)
+        if hasattr(base, "model_io"):        # models with noise and constraints: this step's draws, the constraint out
+            noise, extra["constraint"] = base.model_io(B, dev)
+            keep.append(noise)
+            _lib.check(_lib.lib().gops_b200_plan_set_model_io(plan.handle, _lib.ptr(noise), _lib.ptr(extra["constraint"])))
         _lib.check(_lib.lib().gops_b200_model_step(
             plan.handle, C.byref(b), _lib.ptr(act), _lib.ptr(nobs), _lib.ptr(rew), _lib.ptr(ndone),
             _lib.ptr(extra.get("state")), _lib.ptr(extra.get("ref_points")), _lib.ptr(extra.get("ref_time")),
             _lib.stream_ptr()))
+        if hasattr(base, "model_io"):        # the buffers are this call's: a later call must set its own
+            _lib.check(_lib.lib().gops_b200_plan_set_model_io(plan.handle, None, None))
     extra["_obs_in"] = obs_d if not getattr(top, "_scales_obs", False) else obs_d     # constraint providers read the incoming obs
     next_info = base.make_next_info(info, extra)
     return nobs.to(src), rew.to(src), (ndone != 0).to(src), next_info

@@ -18,6 +18,7 @@ gops/env/env_ocp/resources/ref_traj_model.py:54-232 with the default parameters 
 import math
 from typing import Dict
 
+import numpy as np
 import torch
 
 TWO_PI = 2.0 * math.pi
@@ -88,6 +89,18 @@ def sample_idpendulum(batch, device, seed=0, gen=None) -> Dict[str, torch.Tensor
     high = torch.tensor([5, 0.1, 0.1, 0.3, 0.3, 0.3], dtype=torch.float32, device=device)
     return {"obs": (torch.rand(batch, 6, generator=g, device=device) * 2 - 1) * high,
             "done": torch.zeros(batch, device=device)}
+
+
+def sample_mobilerobot(batch, device, seed=0, gen=None) -> Dict[str, torch.Tensor]:
+    """The data env's uniform reset box (env_ocp/pyth_mobilerobot.py:31-53) with the tracking error of the drawn robot
+    state against the path y = 0 (its `reset`): [y, theta, v - 0.3]."""
+    g = gen or _gen(device, seed)
+    f32 = lambda v: torch.tensor(np.asarray(v, dtype=np.float32), device=device)
+    low = f32([0, -1, -0.6, 0, 0] + [0, 0, 0] + [3.5, -3, np.pi / 2 - 0.3, 0.0, 0])
+    high = f32([2.7, 1, 0.6, 0.3, 0] + [0, 0, 0] + [6, 3, np.pi / 2 + 0.3, 0.5, 0])
+    obs = low + torch.rand(batch, 13, generator=g, device=device) * (high - low)
+    obs[:, 5], obs[:, 6], obs[:, 7] = obs[:, 1], obs[:, 2], obs[:, 3] - np.float32(0.3)
+    return {"obs": obs, "done": torch.zeros(batch, device=device)}
 
 
 def sample_lq(batch, lq_config, device, seed=0, gen=None) -> Dict[str, torch.Tensor]:

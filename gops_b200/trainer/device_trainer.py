@@ -33,6 +33,8 @@ class DeviceStateSampler:
         elif env_id in ("pyth_veh3dofconti", "pyth_veh3dofconti_errcstr"):
             # the errcstr data env inherits pyth_veh3dofconti's reset law (pyth_veh3dofconti_errcstr.py:19)
             self._draw = lambda b: ds.sample_veh3dofconti(b, P, self.device, gen=self.gen)
+        elif env_id == "pyth_mobilerobot":
+            self._draw = lambda b: ds.sample_mobilerobot(b, self.device, gen=self.gen)
         elif env_id == "veh3dof_tracking":
             self._draw = lambda b: ds.sample_veh3dof_tracking(b, P, self.device, gen=self.gen)
         elif env_id == "veh3dof_tracking_detour":

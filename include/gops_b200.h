@@ -41,7 +41,9 @@ enum {
   GOPS_MODEL_IDPENDULUM = 0,      /* env_ocp/env_model/pyth_idpendulum_model.py:199-216           */
   GOPS_MODEL_LQ = 1,              /* env_ocp/resources/lq_base.py:343-354                         */
   GOPS_MODEL_VEH3DOFCONTI = 2,    /* env_ocp/env_model/pyth_veh3dofconti_model.py:91-145          */
-  GOPS_MODEL_VEH3DOF_TRACKING = 3 /* env_gen_ocp/env_model/veh3dof_tracking_model.py:11-102       */
+  GOPS_MODEL_VEH3DOF_TRACKING = 3,/* env_gen_ocp/env_model/veh3dof_tracking_model.py:11-102       */
+  GOPS_MODEL_MOBILEROBOT = 4      /* env_ocp/env_model/pyth_mobilerobot_model.py:61-195: state == obs (13), 2 actions,
+                                     one constraint, obstacle noise (gops_b200_plan_set_model_io)                 */
 };
 
 /* activations                      gops/utils/common_utils.py:26-55 ------------------------- */
@@ -175,7 +177,9 @@ int gops_b200_plan_last_path(const gops_b200_plan* plan);
  *                                     + coef * mean(~feasible * sum_k g^k sum_i max(c_i,0)^2)     fhadp_interior.py:55-84
  * coef = penalty / multiplier of the CURRENT update (the algorithms anneal it on the host).  scalars_out of
  * rollout_grad then carries [0] total loss, [1] the exterior / linear constraint term (mean), [2] #done, [3] #feasible.
- *   mode 4  SPIL (gops/algorithm/spil.py), pyth_veh3dofconti_errcstr on the mma.sync kernel only (coef unused):
+ *   mode 4  SPIL (gops/algorithm/spil.py) on the mma.sync kernel only (coef unused), on pyth_veh3dofconti_errcstr (two
+ *           constraints of the incoming observation) and pyth_mobilerobot (one constraint of the raw next state, done
+ *           samples included; scalars_out [3] is then 0 and w_c1 unused):
  *     INFADP_VALUE plan  spil.py:182-212: loss_v = mean((v(o) - R)^2), R = sum_k g^k r_k + g^n v_target(o_n) WITHOUT the
  *                        (~d) mask; scalars_out = [0] loss_v, [1] mean v(o), [2] / [3] number of trajectories whose
  *                        constraint 0 / 1 stayed <= 0 on every step (the safe counts the controller turns into safe_prob).
@@ -188,6 +192,12 @@ int gops_b200_plan_set_constraint(gops_b200_plan* plan, int mode, float coef);
 /* SPIL policy pass: DEVICE pointer to float[3] = [w_r, w_c0, w_c1] (written by gops_b200_spil_controller), read by every
  * later rollout_grad of this plan.  The pointer must stay valid while the plan uses it. */
 int gops_b200_plan_set_spil_weights(gops_b200_plan* plan, const float* weights);
+/* Models with noise and constraints (GOPS_MODEL_MOBILEROBOT): DEVICE pointers read / written by later calls of this
+ * plan, which must stay valid while the plan uses them.
+ *   noise:          the model's standard-deviation-scaled draws float32(normal(0, (0.03, 0.02))) of the obstacle's (v, w),
+ *                   [horizon][batch][2] for rollout_grad / rollout_trace, [batch][2] for model_step (required on this model)
+ *   constraint_out: [batch][1] info["constraint"] of model_step (0.89 - obstacle distance of the raw next state), or NULL */
+int gops_b200_plan_set_model_io(gops_b200_plan* plan, const float* noise, float* constraint_out);
 /* SPIL's PI multiplier controller (spil.py:257-270), one launch on `stream`, no host sync.  tail: DEVICE float[4] scalars of
  * the value pass (after the gradient exchange, so slots 2 / 3 hold the global safe counts); batch_global: the global batch
  * size.  safe_prob = float32(count) / float32(batch); state: DEVICE double[6] = [delta_i(2), safe_prob_pre(2), lam(2)],

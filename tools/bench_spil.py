@@ -1,6 +1,7 @@
 """Time per update of SPIL on pyth_veh3dofconti_errcstr (value pass, device controller, policy pass, two Adam steps, two
 Polyak averages) at B = 4096 and 2^16, next to INFADP on pyth_veh3dofconti (one PEV plus one PIM update) on the same
-[64, 64] relu nets, forward_step 10, P = 10.  CUDA events around every timed call (each update ends in its scalar
+[64, 64] relu nets, forward_step 10, P = 10; and SPIL on pyth_mobilerobot with the shipped configuration ([64, 64] relu,
+forward_step 25) at B = 1024 and 2^16, with the cost of its per-pass obstacle-noise draws timed on their own.  CUDA events around every timed call (each update ends in its scalar
 read-back, loss_lag = 0), median of 20 after 3 warm-ups; launches per update from gops_b200_launch_count; fused-kernel
 time per pass from the plans' own events (gops_b200_plan_enable_timing) in separate calls.  Prints one JSON line per leg,
 then one with the device and its power limit.
@@ -22,6 +23,7 @@ from gops_b200.create_pkg.create_alg import create_alg  # noqa: E402
 from gops_b200.trainer.device_trainer import DeviceStateSampler  # noqa: E402
 
 BATCHES, WARMUP, REPS = (4096, 1 << 16), 3, 20
+ROBOT_BATCHES, ROBOT_H = (1024, 1 << 16), 25
 
 
 def kwargs(algorithm, env_id):
@@ -34,6 +36,16 @@ def kwargs(algorithm, env_id):
     if algorithm == "SPIL":
         kw.update(forward_step=10, constraint_dim=2, y_error_tol=0.1)
     return kw
+
+
+def robot_kwargs():
+    hi = np.array([0.4, np.pi / 3], np.float32)
+    return dict(env_id="pyth_mobilerobot", algorithm="SPIL", seed=0, trainer="off_serial_trainer", use_gpu=True,
+                action_type="continu", obsv_dim=13, action_dim=2, action_high_limit=hi, action_low_limit=-hi,
+                policy_func_name="DetermPolicy", policy_func_type="MLP", policy_hidden_sizes=[64, 64],
+                policy_hidden_activation="relu", policy_act_distribution="default", policy_learning_rate=3e-4,
+                value_func_name="StateValue", value_func_type="MLP", value_hidden_sizes=[64, 64],
+                value_hidden_activation="relu", value_learning_rate=2e-3, forward_step=ROBOT_H, constraint_dim=1)
 
 
 def timed(step):
@@ -90,6 +102,18 @@ def main():
         two = lambda i: (infadp.local_update(data, 2 * i), infadp.local_update(data, 2 * i + 1))
         report("INFADP PEV+PIM", *timed(two), unit="per PEV+PIM pair", batch=B, kernel_ms=kernel_ms(infadp, two))
         del infadp
+    for B in ROBOT_BATCHES:
+        torch.manual_seed(0)
+        data = DeviceStateSampler("pyth_mobilerobot", "cuda", 1).sample(B)
+        spil = create_alg(**robot_kwargs())
+        model = spil.envmodel.unwrapped
+        # one pass's draws: torch.randn and the std scaling, ROBOT_H * B * 2 floats (8 bytes per sample and step)
+        dev = spil._device()     # the device (and so the generator) the update's own draws use
+        draw_ms, _ = timed(lambda i: model.draw_noise((ROBOT_H, B, 2), dev))
+        report("SPIL mobilerobot", *timed(lambda i: spil.local_update(data, i)), unit="per update", batch=B,
+               kernel_ms=kernel_ms(spil, lambda i: spil.local_update(data, i)), noise_draw_ms_per_pass=round(draw_ms, 4),
+               noise_bytes_per_pass=ROBOT_H * B * 2 * 4)
+        del spil
     try:
         q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
                             str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout.strip()
