@@ -143,6 +143,14 @@ PROTOTYPES = {
     "gops_b200_peer_allreduce": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                            C.c_int32, C.c_double, C.c_double, C.c_double, C.c_double, C.c_void_p]),
     "gops_b200_peer_error": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32)]),
+    "gops_b200_rpi_policy": (C.c_int, [C.c_void_p, C.c_int32, C.c_double, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "gops_b200_rpi_loss_grad": (C.c_int, [C.c_void_p, C.c_int32, C.c_double, C.c_void_p, C.c_void_p, C.c_int64,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "gops_b200_rpi_scratch_floats": (C.c_int64, [C.c_int64]),
+    "gops_b200_rpi_newton": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_double, C.c_double,
+                                       C.c_double, C.c_double, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int64, C.c_void_p,
+                                       C.c_void_p, C.c_void_p]),
 }
 
 _lib = None

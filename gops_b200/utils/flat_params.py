@@ -109,11 +109,27 @@ class FusedAdam(torch.optim.Optimizer):
         if not flat.is_cuda:
             raise RuntimeError("gops_b200.FusedAdam: parameters must live on a CUDA device (no CPU fallback)")
         fp.gather_grads()
+        self._moments(flat)
+        self._step += 1
+        return fp, flat
+
+    def _moments(self, flat):
         if self._m is None or self._m.device != flat.device or self._m.numel() != flat.numel():
             self._m = torch.zeros_like(flat)
             self._v = torch.zeros_like(flat)
-        self._step += 1
-        return fp, flat
+
+    @torch.no_grad()
+    def multi_step_state(self):
+        """(params, exp_avg, exp_avg_sq, steps taken so far, group) for a kernel that takes several Adam steps itself
+        (RPI's Newton iteration, csrc/rpi.cu); `advance(n)` then records the n steps it took."""
+        flat = self.flat_params.sync()
+        if not flat.is_cuda:
+            raise RuntimeError("gops_b200.FusedAdam: parameters must live on a CUDA device (no CPU fallback)")
+        self._moments(flat)
+        return flat, self._m, self._v, self._step, self.param_groups[0]
+
+    def advance(self, n: int):
+        self._step += int(n)
 
     @torch.no_grad()
     def fused_state(self):

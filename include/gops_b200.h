@@ -401,6 +401,35 @@ int gops_b200_peer_allreduce(gops_b200_peer* peer, float* buf, int64_t n, float*
                              double eps, void* stream);
 int gops_b200_peer_error(gops_b200_peer* peer, int32_t* err);
 
+/* RPI (relaxed policy iteration, gops/algorithm/rpi.py) on pyth_oscillatorconti with a StateValue MLP [2 -> 64 -> 64 -> 1]
+ * (hidden activation act: relu / elu / gelu / selu / sigmoid / tanh).  Parameter vectors are the value net's flat
+ * parameters (4417 floats).  gamma_atte: the H-infinity attenuation of the model (the wrapped action bounds are
+ * [-5, 5] and [-1/gamma_atte, 1/gamma_atte]).
+ *
+ * ApproxContainer.action_and_adversary (rpi.py:90-103) and the model's best_act / worst_adv
+ * (pyth_oscillatorconti_model.py:772-815): act_out[b] = raw (a, w) = (-0.5 x0 p1, 0.5 / gamma_atte^2 x1 p1), p = dV/dx of
+ * the target net at obs[b]; any batch. */
+int gops_b200_rpi_policy(const float* target_params, int32_t act, double gamma_atte, const float* obs, int64_t batch,
+                         float* act_out, void* stream);
+/* RPI.__compute_loss / __calculate_hamiltonian (rpi.py:218-287) once: loss = mean_b |c + dV/dx . f| of the wrapped model
+ * at (obs[b], act_in[b] = raw (a, w)); grad_out[4417] = d loss / d params, loss_out[1].  batch: a multiple of 64;
+ * scratch: gops_b200_rpi_scratch_floats(batch) floats. */
+int gops_b200_rpi_loss_grad(const float* params, int32_t act, double gamma_atte, const float* obs, const float* act_in,
+                            int64_t batch, float* scratch, float* grad_out, float* loss_out, void* stream);
+int64_t gops_b200_rpi_scratch_floats(int64_t batch);
+/* One Newton iteration, RPI.local_update (rpi.py:174-215) with RPI.sample (:289-327), in ONE launch of a thread-block
+ * cluster of batch / 64 CTAs (batch a multiple of 64, at most 512; threshold0/1: the model's state_threshold): H_before at set_state, then per inner step sample,
+ * loss and gradient, cluster reduction, Adam (arguments as gops_b200_adam_step, steps step0 + 1, step0 + 2, ...) and
+ * H_after, until H_after <= 0.88 H_before or max_steps steps; then target <- params.
+ *   state [batch][2] sampler states, counter [1] the model's step_per_episode, both updated; max_step [batch];
+ *   draws [rows][batch][2] reset() draws: row 0 is set_state, row n the reset draw of inner step n;
+ *   out [8]: [0] steps n, [1] loss of the last step, [2] H_before, [3] H_after, [4] 1 if the loop stopped because the
+ *   draws ran out; trace: NULL or [max_steps][2] (loss, H_after) per inner step. */
+int gops_b200_rpi_newton(float* params, float* target, float* exp_avg, float* exp_avg_sq, int64_t step0, double lr,
+                         double beta1, double beta2, double eps, int32_t act, double gamma_atte, double threshold0, double threshold1,
+                         float* state, const int32_t* max_step, int32_t* counter, const float* draws, int32_t rows,
+                         int32_t max_steps, int64_t batch, float* out, float* trace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
